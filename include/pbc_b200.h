@@ -194,8 +194,13 @@ const char *pbc_b200_last_error(void);
  *          multiplier in registers, 3 = product-scanning squaring in registers.  muls = threads * iters.
  *   imad : IMAD.WIDE.U32 issue-rate probe, 32 * iters instructions per thread: the faster of two
  *          kernels, four independent carry chains of eight and eight carry-free chains of four
- *          (data-dependent multiplicands in both). */
+ *          (data-dependent multiplicands in both).
+ *   fpmul_smem (type a): fpmul mode 1 with smem_bytes of dynamic shared memory per 128-thread block
+ *          (at least the 16 KB it uses), so that it runs at the occupancy of a kernel with that
+ *          footprint.  One full wave: *blocks_per_sm (the device's occupancy for that size) times the
+ *          multiprocessor count blocks.  muls = blocks * 128 * iters. */
 double pbc_b200_bench_fpmul(pbc_b200_pairing_t *p, int mode, int blocks, int iters, int reps);
+double pbc_b200_bench_fpmul_smem(pbc_b200_pairing_t *p, int smem_bytes, int iters, int reps, int *blocks_per_sm);
 double pbc_b200_bench_imad(int blocks, int threads, int iters, int reps);
 
 /* Per-stage device timing of the device-buffer path (bench.py roofline): when enabled,

@@ -62,6 +62,8 @@ lib.pbc_b200_kernel_launches.restype = C.c_uint64
 lib.pbc_b200_last_error.restype = C.c_char_p
 lib.pbc_b200_bench_fpmul.argtypes = [_P, C.c_int, C.c_int, C.c_int, C.c_int]
 lib.pbc_b200_bench_fpmul.restype = C.c_double
+lib.pbc_b200_bench_fpmul_smem.argtypes = [_P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
+lib.pbc_b200_bench_fpmul_smem.restype = C.c_double
 lib.pbc_b200_bench_imad.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
 lib.pbc_b200_bench_imad.restype = C.c_double
 lib.pbc_b200_set_stage_profiling.argtypes = [_P, C.c_int]

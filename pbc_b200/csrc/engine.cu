@@ -190,6 +190,20 @@ struct Job {
 
 static size_t cc_table_bytes(const pbc_b200_pairing_s* p);
 
+// PBC_A_SLOTS: slots of the type A Miller kernel of pairings and unshared products.  9 (default):
+// k_a_miller9, three 128-thread blocks per SM; 7: k_a_miller7, four blocks -- 2.5 % fewer cycles per
+// pairing, but on a power-capped H100 the clock drops more than that (DESIGN.md 3.8); 14: k_a_miller of
+// round 1, two blocks.  7 and 14 are kept for A/B runs.  Products that share an accumulator run
+// k_a_miller9_shared in every setting.
+#ifndef PBC_A_SLOTS
+#define PBC_A_SLOTS 9
+#endif
+static_assert(PBC_A_SLOTS == 7 || PBC_A_SLOTS == 9 || PBC_A_SLOTS == 14, "PBC_A_SLOTS: 7, 9 or 14");
+// threads of the type A Miller grid for n pairings (whole blocks)
+static size_t a_miller_cols(size_t n) { return (n + kBlockMiller - 1) / kBlockMiller * kBlockMiller; }
+// the g array of k_a_miller7 (f^2 and g0 + g1, one column per thread of its grid); the other kernels need none
+static size_t a_miller_g_bytes(size_t n) { return PBC_A_SLOTS == 7 ? 3 * 64 * a_miller_cols(n) : 0; }
+
 // workspace bytes for n_out outputs of `job`
 static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out) {
   if (p->type == '1') {
@@ -201,10 +215,12 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
   }
   if (p->type == 'a') {
     const size_t fq = 64;
-    // f [2], dprod, prefix, save [5] (V1, f1), qm [2] (Montgomery-form Q of the nine-slot Miller kernel)
-    if (job.mode == kSingle) return n_out * (2 + 1 + 1 + 5 + 2) * fq;
+    // f [2], dprod, prefix, save [5] (V1, f1), qm [2] (Montgomery-form Q of the nine- and seven-slot
+    // Miller kernels), then the g array of the seven-slot kernel
+    if (job.mode == kSingle) return n_out * (2 + 1 + 1 + 5 + 2) * fq + a_miller_g_bytes(n_out);
     // products: + vj [3] per pair (V of the pairs that share an accumulator, k_a_miller9_shared)
-    if (job.mode == kProd) return n_out * job.k * (2 + 1 + 5 + 2 + 3) * fq + n_out * (2 + 1 + 1) * fq;
+    if (job.mode == kProd)
+      return n_out * job.k * (2 + 1 + 5 + 2 + 3) * fq + n_out * (2 + 1 + 1) * fq + a_miller_g_bytes(n_out * job.k);
     return n_out * (2 + 1 + 1) * fq + (size_t)(3 * (p->a.exp2 + 1) * kNA + 4) * 4;
   }
   // types f, d: Miller values [W][n] words + one flag word each; products add the reduced arrays
@@ -775,12 +791,8 @@ static cudaError_t allow_smem(K kernel, size_t bytes) {
 }
 
 static constexpr size_t kSmemAMiller = (size_t)kASlots * 64 * kBlockMiller;
-// PBC_A_SLOTS9 = 1 (default): the nine-slot Miller kernel, three 128-thread blocks per SM; 0: the
-// 14-slot kernel of round 1 (two blocks per SM) -- kept for A/B runs
-#ifndef PBC_A_SLOTS9
-#define PBC_A_SLOTS9 1
-#endif
 static constexpr size_t kSmemAMiller9 = (size_t)kA9Slots * 64 * kBlockMiller;
+static constexpr size_t kSmemAMiller7 = (size_t)kA7Slots * 64 * kBlockMiller;
 // PBC_F_SLOTS = 1 (default): type F Miller loop on the shared-memory slot machine (pairing_f_slots.cuh)
 // where the parameters allow it; 0: the round-1 kernel (local-memory frames)
 #ifndef PBC_F_SLOTS
@@ -844,6 +856,7 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
     if (p->type == 'a') {
       CUDA_OK(allow_smem(k_a_miller<kBlockMiller>, kSmemAMiller));
       CUDA_OK(allow_smem(k_a_miller9<kBlockMiller>, kSmemAMiller9));
+      CUDA_OK(allow_smem(k_a_miller7<kBlockMiller>, kSmemAMiller7));
       CUDA_OK(allow_smem(k_a_miller9_shared<kBlockMiller>, kSmemAMiller9));
       CUDA_OK(allow_smem(k_a_finalexp<kBlockFinal>, kSmemAFinal));
       CUDA_OK(allow_smem(k_batch_invert<kNA, true, kBlockInv>, kSmemInv16));
@@ -954,6 +967,15 @@ static size_t inv_threads(const pbc_b200_pairing_s* p, size_t n, size_t per_sm) 
   return n < t ? n : t;
 }
 
+// the type A Miller kernel PBC_A_SLOTS selects, one thread per pairing; g: [3][4][a_miller_cols(n)] uint4
+static void launch_a_miller(const uint8_t* P, const uint8_t* Q, uint4* f, uint4* dprod, uint4* save, uint4* qm,
+                            uint4* g, size_t n, cudaStream_t st) {
+  unsigned gm = (unsigned)(a_miller_cols(n) / kBlockMiller);
+  if (PBC_A_SLOTS == 7) k_a_miller7<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller7, st>>>(P, Q, f, dprod, save, qm, g, n);
+  else if (PBC_A_SLOTS == 9) k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(P, Q, f, dprod, save, qm, n);
+  else k_a_miller<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller, st>>>(P, Q, f, dprod, save, n);
+}
+
 // ------------------------------------------------------------------------------------------
 // enqueue one batch of n_out outputs of `job`, device buffers, on `st`.  ws: ws_bytes() bytes.
 // ------------------------------------------------------------------------------------------
@@ -1023,9 +1045,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       prefix = dprod + 4 * n;                    // [4][n]
       uint4* save = prefix + 4 * n;              // [5][4][n]
       uint4* qm = save + 20 * n;                 // [2][4][n]
-      unsigned gm = (unsigned)((n + kBlockMiller - 1) / kBlockMiller);
-      if (PBC_A_SLOTS9) k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, f, dprod, save, qm, n);
-      else k_a_miller<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller, st>>>(d_in1, d_in2, f, dprod, save, n);
+      uint4* g = qm + 8 * n;                     // a_miller_g_bytes(n)
+      launch_a_miller(d_in1, d_in2, f, dprod, save, qm, g, n, st);
       LAUNCHED();
     } else if (job.mode == kProd) {
       size_t m = n * job.k;
@@ -1037,11 +1058,12 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       f = vj + 12 * m;                           // [2][4][n]
       dprod = f + 8 * n;
       prefix = dprod + 4 * n;
+      uint4* g = prefix + 4 * n;                 // a_miller_g_bytes(m)
       // pairs per thread sharing one accumulator: the largest divisor of k not above the handle's setting
       // that still leaves four waves of threads (sharing divides the thread count, and with too few
       // threads the GPU idles)
       size_t share = 1;
-      if (PBC_A_SLOTS9) {
+      if (PBC_A_SLOTS != 14) {
         const size_t wave = cur_sms(p) * 3 * kBlockMiller;
         for (size_t c = (size_t)p->prod_share; c > 1; c--)
           if (job.k % c == 0 && (m / c >= 4 * wave || p->prod_share_forced)) { share = c; break; }
@@ -1053,9 +1075,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
         unsigned gs = (unsigned)((mm + kBlockMiller - 1) / kBlockMiller);
         k_a_miller9_shared<kBlockMiller><<<gs, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, fi, di, save, qm, vj, mm, share);
       } else {
-        unsigned gm = (unsigned)((m + kBlockMiller - 1) / kBlockMiller);
-        if (PBC_A_SLOTS9) k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, fi, di, save, qm, m);
-        else k_a_miller<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller, st>>>(d_in1, d_in2, fi, di, save, m);
+        launch_a_miller(d_in1, d_in2, fi, di, save, qm, g, m, st);
       }
       LAUNCHED();
       unsigned gp = (unsigned)((n + kBlockProd - 1) / kBlockProd);
@@ -1478,12 +1498,14 @@ void* pbc_b200_host_alloc(size_t bytes) {
 void pbc_b200_host_free(void* ptr) { if (ptr) cudaFreeHost(ptr); }
 
 // ---- roofline probes ----
-double pbc_b200_bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters, int reps) {
+// smem > 0 (type a, the slot multiplier of mode 1 only): launch with that much dynamic shared memory per block
+static double bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters, int reps, size_t smem) {
   if (!p) { fail("null argument"); return -1; }
   if (p->type == '1') { fail("bench_fpmul: not built for type a1"); return -1; }
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || ctx_prepare(p, dev)) return -1;
   const int threads = 128;
+  if (smem < 2 * 64 * 128) smem = 2 * 64 * 128;
   size_t T = (size_t)blocks * threads;
   int N = p->nlimbs;
   uint32_t *in = nullptr, *out = nullptr;
@@ -1506,7 +1528,7 @@ double pbc_b200_bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int ite
       else if (mode == 3) k_fpmul_chain<kNA, true, 2><<<blocks, threads, 0, st>>>(out, in, iters);
       else if (mode == 4) k_fpmul_slots<kNA, true, 128, 1><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else if (mode == 5) k_fpmul_slots<kNA, true, 128, 2><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
-      else k_fpmul_slots<kNA, true, 128, 0><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
+      else k_fpmul_slots<kNA, true, 128, 0><<<blocks, threads, smem, st>>>(out, in, iters);
     } else {
       k_fqmul_chain<<<blocks, threads, 0, st>>>(out, in, iters, mode == 3 ? 1 : 0);
     }
@@ -1525,6 +1547,31 @@ double pbc_b200_bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int ite
   cudaFree(in); cudaFree(out);
   if (err != cudaSuccess) { fail("bench_fpmul: %s", cudaGetErrorString(err)); return -1; }
   return ms / reps;
+}
+double pbc_b200_bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters, int reps) {
+  return bench_fpmul(p, mode, blocks, iters, reps, 0);
+}
+double pbc_b200_bench_fpmul_smem(pbc_b200_pairing_t* p, int smem_bytes, int iters, int reps, int* blocks_per_sm) {
+  if (!p || !blocks_per_sm || smem_bytes < 0) { fail("null or negative argument"); return -1; }
+  if (p->type != 'a') { fail("bench_fpmul_smem: type a only"); return -1; }
+#ifdef PBC_HOST_SIM
+  (void)iters; (void)reps;
+  fail("bench_fpmul_smem: needs a GPU");
+  return -1;
+#else
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || ctx_prepare(p, dev)) return -1;
+  const size_t smem = smem_bytes < 2 * 64 * 128 ? 2 * 64 * 128 : (size_t)smem_bytes;
+  auto kern = k_fpmul_slots<kNA, true, 128, 0>;
+  int occ = 0;
+  cudaError_t e = allow_smem(kern, smem);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 128, smem);
+  if (e != cudaSuccess) { fail("bench_fpmul_smem: %s", cudaGetErrorString(e)); return -1; }
+  *blocks_per_sm = occ;
+  if (occ < 1) { fail("bench_fpmul_smem: %d bytes per block do not fit an SM", smem_bytes); return -1; }
+  // one full wave: every block resident for the whole run
+  return bench_fpmul(p, 1, occ * (int)p->ctx[dev].sms, iters, reps, smem);
+#endif
 }
 
 // the faster of the two IMAD.WIDE.U32 probes (common_kernels.cuh), each warmed up, then timed over reps launches

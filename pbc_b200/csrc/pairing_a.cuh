@@ -328,34 +328,40 @@ __device__ __forceinline__ void a_fmul_2t(int f0, int f1, int l0, int l1, int t0
   O::copy(f0, t1);
 }
 
-// f *= the chord through V = (nX, nY, nZ) and the saved V1 = (X1, Y1, Z1) of pair `idx`, evaluated at
-// phi(Q); V is consumed.  Weight-(1,2) coordinates, scaled by Z^2 Z1^2 (compute_abc_line :114-130).
+// The chord through V = (x, y, z) and the saved V1 = (X1, Y1, Z1) of pair `idx`, evaluated at phi(Q):
+// Re l into t3, Im l into t2; V is consumed.  Weight-(1,2) coordinates, scaled by Z^2 Z1^2
+// (compute_abc_line :114-130).
+template <class O>
+__device__ __forceinline__ void a_chord_line(int x, int y, int z, int t0, int t1, int t2, int t3, const uint4* save,
+                                             const uint4* qx, const uint4* qy, size_t n, size_t idx) {
+  //   a = Y Z1^2 - Y1 Z^2,  b = Z Z1 (X1 Z - X Z1),  c = X Z Y1 - Y X1 Z1
+  O::ld_global(t0, save, 2, n, idx);           // Z1
+  O::ld_global(t1, save, 0, n, idx);           // X1
+  O::mulp(t2, t1, z);                           // X1 Z
+  O::mulp(t3, x, t0);                           // X Z1
+  O::sub(t2, t2, t3);
+  O::mulp(t2, t2, z);
+  O::mulp(t2, t2, t0);                          // b
+  O::mulp(t3, x, z);                            // X Z               (last use of X)
+  O::ld_global(x, save, 1, n, idx);            // Y1
+  O::mulp(t3, t3, x);                           // X Z Y1
+  O::mulp(t1, t1, t0);                          // X1 Z1
+  O::mulp(t1, t1, y);                           // Y X1 Z1
+  O::sub(t3, t3, t1);                           // c
+  O::sqr(t0, t0);                               // Z1^2
+  O::mulp(t0, t0, y);                           // Y Z1^2
+  O::sqr(t1, z);                                // Z^2
+  O::mulp(t1, t1, x);                           // Y1 Z^2
+  O::sub(t0, t0, t1);                           // a
+  O::mulg(t0, t0, qx, n);
+  O::sub(t3, t3, t0);                           // Re l = c - a Qx
+  O::mulg(t2, t2, qy, n);                       // Im l = b Qy
+}
+// f *= the chord through V = (nX, nY, nZ) and the saved V1 of pair `idx`
 template <class O>
 __device__ __forceinline__ void a_chord_9(const uint4* save, const uint4* qx, const uint4* qy, size_t n, size_t idx) {
-  //   a = Y Z1^2 - Y1 Z^2,  b = Z Z1 (X1 Z - X Z1),  c = X Z Y1 - Y X1 Z1
-  O::ld_global(nT0, save, 2, n, idx);          // Z1
-  O::ld_global(nT1, save, 0, n, idx);          // X1
-  O::mulp(nT2, nT1, nZ);                         // X1 Z
-  O::mulp(nT3, nX, nT0);                         // X Z1
-  O::sub(nT2, nT2, nT3);
-  O::mulp(nT2, nT2, nZ);
-  O::mulp(nT2, nT2, nT0);                        // b
-  O::mulp(nT3, nX, nZ);                          // X Z               (last use of X)
-  O::ld_global(nX, save, 1, n, idx);           // Y1
-  O::mulp(nT3, nT3, nX);                         // X Z Y1
-  O::mulp(nT1, nT1, nT0);                        // X1 Z1
-  O::mulp(nT1, nT1, nY);                         // Y X1 Z1
-  O::sub(nT3, nT3, nT1);                        // c
-  O::sqr(nT0, nT0);                             // Z1^2
-  O::mulp(nT0, nT0, nY);                         // Y Z1^2
-  O::sqr(nT1, nZ);                              // Z^2
-  O::mulp(nT1, nT1, nX);                         // Y1 Z^2
-  O::sub(nT0, nT0, nT1);                        // a
-  O::mulg(nT0, nT0, qx, n);
-  O::sub(nT3, nT3, nT0);                        // Re l = c - a Qx
-  O::mulg(nT2, nT2, qy, n);                     // Im l = b Qy
+  a_chord_line<O>(nX, nY, nZ, nT0, nT1, nT2, nT3, save, qx, qy, n, idx);
   a_fmul_2t<O>(nF0, nF1, nT3, nT2, nT0, nT1);
-
 }
 
 // f, dprod, save as for k_a_miller; qm: [2][4][n] uint4 scratch (Montgomery-form Q)
@@ -422,6 +428,142 @@ k_a_miller9(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4*
   O::st_global(f, 0, n, idx, nF0);
   O::st_global(f, 1, n, idx, nF1);
   O::st_global(dprod, 0, n, idx, nT0);
+}
+
+// ---------------------------------------------------------------------------------------------
+// The same Miller loop on SEVEN slots.  g = f^2 and g0 + g1 go to a limb-major global array as soon as
+// they are computed, like Q, and the products f' = g l take them from there (Ops::mulg), so f needs no
+// slot during the line and doubling part.  The step of k_a_miller9, with the same products (11 M + 6 S),
+// on X, Y, Z and four temporaries; at most seven values are live (X, Y, Z, U, B, A', T).  f' and Y' end
+// in other slots than f and Y started in: the slot numbers are renamed every step instead of copied.
+// 7 x 64 B x 128 threads = 56 KB per block: FOUR blocks = 16 warps per SM (plus the 1 KB the runtime
+// reserves per block, exactly the 228 KB of an H100 SM).  Off by default (engine.cu, PBC_A_SLOTS): 2.5 %
+// fewer cycles than k_a_miller9, but a power-capped H100 lowers its clock by more (DESIGN.md 3.8).
+// ---------------------------------------------------------------------------------------------
+enum A7Slot { sX, sZ, sY0, sF00, sF10, sT00, sT10, kA7Slots };
+
+// one step.  On entry f = (f0, f1), V = (sX, y, sZ), t0 and t1 free; on exit the same for f', 2V.
+// g: this thread's column of the [3][4][ng] array that takes g0, g1 and g0 + g1.
+template <class O>
+__device__ __forceinline__ void a_double_step_7(int& y, int& f0, int& f1, int& t0, int& t1, uint4* g, size_t ng,
+                                                const uint4* qx, const uint4* qy, size_t n) {
+  const int a = f0, b = f1, c = t0, d = t1;
+  O::template mul2<true>(c, f0, f1, f0, f1);         // g0 = (f0 + f1)(f0 - f1)
+  O::mulx(d, f0, f1, O::MX_ADD_A, f0, 0, nullptr, 0);   // g1 = 2 f0 f1
+  O::add(a, c, d);
+  O::st_global(g, 0, ng, 0, c);
+  O::st_global(g, 1, ng, 0, d);
+  O::st_global(g, 2, ng, 0, a);                      // g0 + g1       (all four temporaries are free)
+  O::sqr(a, sX);                                     // A
+  O::sqr(b, y);                                      // B
+  O::sqr(c, sZ);                                     // C
+  O::sub(d, a, c);                                   // T = A - C
+  O::add(c, a, c);                                   // A' = A + C
+  O::dbl(a, c);
+  O::add(a, a, d);                                   // U = 3A + C
+  O::mulp(a, a, sZ);
+  O::mulg(a, a, qx, n);                              // U Z Qx
+  O::mulp(sX, sX, d);                                // X T
+  O::add(a, a, sX);                                  // Re l                   (X slot is free)
+  O::sqr(sX, d);                                     // X' = T^2
+  O::sqr(c, c);
+  O::dbl(c, c);
+  O::sub(c, c, sX);                                  // E = 2 A'^2 - X'
+  O::add(d, d, y);
+  O::sqr(d, d);
+  O::sub(d, d, b);
+  O::sub(d, d, sX);                                  // F = (T + Y)^2 - B - X'
+  O::mulp(c, c, d);                                  // Y'
+  O::mulp(d, y, sZ);
+  O::dbl(d, d);
+  O::mulg(d, d, qy, n);                              // Im l = 2 Y Z Qy
+  O::dbl(sZ, b, 2);                                  // Z' = 4 B
+  O::mulx(b, a, 0, O::MX_ADD_A | O::MX_GLOBAL_B, d, 0, g + 8 * ng, ng);   // (Re l + Im l)(g0 + g1)
+  O::mulg(a, a, g, ng);                              // g0 Re l
+  O::mulg(d, d, g + 4 * ng, ng);                     // g1 Im l
+  O::sub(y, a, d);                                   // f0'
+  O::sub(b, b, a);
+  O::sub(b, b, d);                                   // f1'
+  f0 = y; y = c; f1 = b; t0 = a; t1 = d;
+}
+
+// f, dprod, save, qm as for k_a_miller9; g: [3][4][ng] uint4 scratch, ng = n rounded up to BLOCK: every
+// thread, the padding threads of the last block included, owns a column
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK, 4)
+k_a_miller7(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4* __restrict__ f,
+            uint4* __restrict__ dprod, uint4* __restrict__ save, uint4* __restrict__ qm, uint4* __restrict__ g,
+            size_t n) {
+  using O = Ops<kNA, true, BLOCK>;
+  size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
+  const size_t ng = (size_t)gridDim.x * BLOCK;
+  uint4* gcol = g + idx;
+#if PBC_A_LOCKSTEP
+  const bool live = idx < n;                 // every thread runs the loop: block-wide barrier inside
+  if (!live) idx = 0;
+#else
+  if (idx >= n) return;
+  const bool live = true;
+#endif
+  int y = sY0, f0 = sF00, f1 = sF10, t0 = sT00, t1 = sT10;
+  bool okP = a_load_point<O>(sX, y, t0, t1, P + idx * (2 * kWA));
+  bool okQ = a_load_point<O>(f0, f1, t0, t1, Q + idx * (2 * kWA));
+  bool valid = okP && okQ;
+  if (live) {
+    O::st_global(qm, 0, n, idx, f0);
+    O::st_global(qm, 1, n, idx, f1);
+  }
+  const uint4* qx = qm + idx;
+  const uint4* qy = qm + 4 * n + idx;
+
+  O::set_const(sZ, c_fp.one);
+  O::set_const(f0, c_fp.one);
+  uint32_t zero[kNA] = {0};
+  O::st(f1, zero);
+
+  const int exp1 = c_a.exp1, exp2 = c_a.exp2;
+  for (int i = 0; i < exp2; i++) {
+#if PBC_A_LOCKSTEP
+    __syncthreads();
+#endif
+    if (i == exp1 && live) {
+      // V1 = +-V, f1 = f or conj(f) ~ 1/f   (ecc/a_param.c:1162-1169)
+      if (c_a.sign1 < 0) { O::neg(t0, y); O::neg(t1, f1); }
+      else               { O::copy(t0, y); O::copy(t1, f1); }
+      O::st_global(save, 0, n, idx, sX);
+      O::st_global(save, 1, n, idx, t0);
+      O::st_global(save, 2, n, idx, sZ);
+      O::st_global(save, 3, n, idx, f0);
+      O::st_global(save, 4, n, idx, t1);
+    }
+    a_double_step_7<O>(y, f0, f1, t0, t1, gcol, ng, qx, qy, n);
+  }
+  if (!live) return;
+
+  // f *= chord, then f *= f1 (the order of the two factors does not change the product).  f is parked in
+  // the output array while the chord takes four temporaries.
+  O::st_global(f, 0, n, idx, f0);
+  O::st_global(f, 1, n, idx, f1);
+  a_chord_line<O>(sX, y, sZ, f0, f1, t0, t1, save, qx, qy, n, idx);    // Re l in t1, Im l in t0
+  O::ld_global(sX, f, 0, n, idx);
+  O::ld_global(y, f, 1, n, idx);
+  a_fmul_2t<O>(sX, y, t1, t0, f0, f1);
+  O::ld_global(t0, save, 3, n, idx);
+  O::ld_global(t1, save, 4, n, idx);
+  a_fmul_2t<O>(sX, y, t0, t1, f0, f1);
+  f0 = sX;
+  f1 = y;
+
+  // D = (f0^2 + f1^2) f0 f1;  invalid inputs publish D = 0 (-> identity)
+  O::sqr(t0, f0);
+  O::sqr(t1, f1);
+  O::add(t0, t0, t1);
+  O::mulp(t1, f0, f1);
+  O::mulp(t0, t0, t1);
+  if (!valid) O::st(t0, zero);
+  O::st_global(f, 0, n, idx, f0);
+  O::st_global(f, 1, n, idx, f1);
+  O::st_global(dprod, 0, n, idx, t0);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -702,47 +844,48 @@ k_a_pp_apply(const uint32_t* __restrict__ tab, const uint8_t* __restrict__ Q, ui
   O::st_global(dprod, 0, n, idx, qT0);
 }
 
-// slot map of the final-exponentiation kernel
-enum AFSlot { fF0, fF1, fD, fN, fP, fV0, fV1, fT0, fTWO, kAFSlots };
+// slot map of the final-exponentiation kernel: the Lucas ladder keeps V_0, V_1 and P, plus W = N^2 Dinv
+// for the end; the constant 2 is read from c_a.  4 x 64 B x 128 threads = 32 KB per block: six blocks
+// (24 warps) per SM.
+enum AFSlot { fV0, fV1, fP, fW, kAFSlots };
 
 // out: n * 128 bytes, wire format of F_q^2 (arith/fieldquadratic.c:323-329: x || y).
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK)
+__global__ void __launch_bounds__(BLOCK, 6)
 k_a_finalexp(const uint4* __restrict__ f, const uint4* __restrict__ dinv, uint8_t* __restrict__ out,
              size_t n) {
   using O = Ops<kNA, true, BLOCK>;
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
-  O::ld_global(fF0, f, 0, n, idx);
-  O::ld_global(fF1, f, 1, n, idx);
-  O::ld_global(fD, dinv, 0, n, idx);
-  bool identity = O::is_zero(fD);
-  O::set_const(fTWO, c_a.two);
-  // N = f0^2 + f1^2, W = f0 f1;  1/N = Dinv W;  P = 2 (f0^2 - f1^2) / N
-  O::sqr(fV0, fF0);
-  O::sqr(fV1, fF1);
-  O::add(fN, fV0, fV1);
-  O::sub(fP, fV0, fV1);
-  O::dbl(fP, fP);
-  O::mul(fT0, fF0, fF1);
-  O::mul(fT0, fT0, fD);
-  O::mul(fP, fP, fT0);
+  O::ld_global(fV0, f, 0, n, idx);
+  O::ld_global(fV1, f, 1, n, idx);
+  O::ld_global(fW, dinv, 0, n, idx);
+  bool identity = O::is_zero(fW);
+  // N = f0^2 + f1^2;  1/N = Dinv f0 f1;  P = 2 (f0^2 - f1^2) / N;  W = N^2 Dinv
+  O::mul(fP, fV0, fV1);
+  O::mul(fP, fP, fW);                       // 1/N
+  O::sqr(fW, fV1);
+  O::sqr(fV1, fV0);
+  O::sub(fV0, fV1, fW);
+  O::add(fV1, fV1, fW);                     // N
+  O::dbl(fV0, fV0);
+  O::mul(fP, fP, fV0);                      // P
+  O::sqr(fW, fV1);
+  O::mulg(fW, fW, dinv + idx, n);           // W (Dinv read again inside the call: no registers held)
   // Lucas ladder, lucas_odd (ecc/a_param.c:226-262): V_0 = 2, V_1 = P
-  O::copy(fV0, fTWO);
+  O::set_const(fV0, c_a.two);
   O::copy(fV1, fP);
   for (int j = (int)c_a.hbits - 1; j >= 0; j--) {
     bool bit = j > 0 && ((c_a.h[j >> 5] >> (j & 31)) & 1u);   // last step takes the clear branch
     int d = bit ? fV0 : fV1, s = bit ? fV1 : fV0;
     O::mulsub(d, fV0, fV1, fP);
-    O::sqrsub(s, s, fTWO);
+    O::sqrsub(s, s, c_a.two);
   }
-  // out0 = V_h / 2;  out1 = (2 V_{h+1} - P V_h) N^2 Dinv / 8
+  // out0 = V_h / 2;  out1 = (2 V_{h+1} - P V_h) W / 8
   O::dbl(fV1, fV1);
-  O::mul(fT0, fP, fV0);
-  O::sub(fV1, fV1, fT0);
-  O::sqr(fN, fN);
-  O::mul(fN, fN, fD);
-  O::mul(fV1, fV1, fN);
+  O::mul(fP, fP, fV0);
+  O::sub(fV1, fV1, fP);
+  O::mul(fV1, fV1, fW);
   O::halve(fV1, fV1, 3);
   O::halve(fV0, fV0);
 

@@ -67,7 +67,7 @@ struct Ops {
     fp_sqr<N, FULL>(x, x);
     st(d, x);
   }
-  // ---- ONE multiplier routine for the kernels that need operand variants (k_a_miller9) ----
+  // ---- ONE multiplier routine for the kernels that need operand variants (k_a_miller9, k_a_miller7) ----
   // d = x * y with  x = a [+ a2],  y = b [+ b2 | - b2]  or  y = the element at g (limb-major global
   // array, vectors n apart: a value used once or twice per loop iteration lives in L2 instead of a
   // slot).  All branches are warp-uniform.  One copy of the 528-product body instead of one per
@@ -125,12 +125,13 @@ struct Ops {
     fp_sub<N>(x, x, y);
     st(d, x);
   }
-  // d = a^2 - c
-  static __device__ __noinline__ void sqrsub(int d, int a, int c) {
+  // d = a^2 - c, c a constant (not a slot: one slot fewer for the Lucas ladder of k_a_finalexp)
+  static __device__ __noinline__ void sqrsub(int d, int a, const uint32_t* c) {
     uint32_t x[N], y[N];
     ld(x, a);
     fp_sqr<N, FULL>(x, x);
-    ld(y, c);
+#pragma unroll
+    for (int k = 0; k < N; k++) y[k] = c[k];
     fp_sub<N>(x, x, y);
     st(d, x);
   }

@@ -293,6 +293,14 @@ class Pairing:
             raise PairingError(last_error())
         return ms
 
+    def bench_fpmul_smem(self, smem_bytes: int, iters: int, reps: int) -> tuple[float, int]:
+        """(ms, blocks per SM): the slot multiplier at the occupancy of smem_bytes per block, one full wave"""
+        bps = C.c_int(0)
+        ms = lib.pbc_b200_bench_fpmul_smem(self._h, smem_bytes, iters, reps, C.byref(bps))
+        if ms < 0:
+            raise PairingError(last_error())
+        return ms, bps.value
+
 
 class PairingPP:
     """pairing_pp_t (include/pbc_pairing.h:54-89): init once, apply many times, clear"""

@@ -191,7 +191,8 @@ const char *pbc_b200_last_error(void);
  *   fpmul: every thread runs `iters` dependent Montgomery multiplications modulo this pairing's
  *          base-field prime; mode 0 = operand-scanning multiplier in registers, 1 = the multiplier
  *          the kernels use, through the shared-memory slot machine, 2 = product-scanning
- *          multiplier in registers, 3 = product-scanning squaring in registers.  muls = threads * iters.
+ *          multiplier in registers, 3 = the squaring the kernels use, in registers, 6 (type a) = that
+ *          squaring through the slot machine.  muls = threads * iters.
  *   imad : IMAD.WIDE.U32 issue-rate probe, 32 * iters instructions per thread: the faster of two
  *          kernels, four independent carry chains of eight and eight carry-free chains of four
  *          (data-dependent multiplicands in both).

@@ -64,7 +64,7 @@ __global__ void k_fpmul_chain(uint32_t* __restrict__ out, const uint32_t* __rest
   for (int i = 0; i < iters; i++) {
     if (IMPL == 0) mont_mul<N, FULL>(a, a, b);
     else if (IMPL == 1) mont_mul_ps<N, FULL>(a, a, b);
-    else mont_sqr_ps<N, FULL>(a, a);
+    else fp_sqr<N, FULL>(a, a);
   }
 #pragma unroll
   for (int k = 0; k < N; k++) out[k * T + t] = a[k];
@@ -72,7 +72,7 @@ __global__ void k_fpmul_chain(uint32_t* __restrict__ out, const uint32_t* __rest
 
 // Same chain through the shared-memory slot machine (what the pairing kernels execute).
 // MIX 0: multiplications only; 1: one multiplication + one addition per step as separate calls (the
-// Miller loop's mix is 19 : 22); 2: the same work as one fused call.
+// Miller loop's mix is 19 : 22); 2: the same work as one fused call; 3: squarings only (O::sqr).
 template <int N, bool FULL, int BLOCK, int MIX>
 __global__ void __launch_bounds__(BLOCK)
 k_fpmul_slots(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int iters) {
@@ -85,7 +85,8 @@ k_fpmul_slots(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int i
   for (int i = 0; i < iters; i++) {
     if (MIX == 0) O::mul(0, 0, 1);
     else if (MIX == 1) { O::mul(0, 0, 1); O::add(0, 0, 1); }
-    else O::fmul(0, 0, 1, O::F_ADD_C1(1), 0, 0, 1, 0);
+    else if (MIX == 2) O::fmul(0, 0, 1, O::F_ADD_C1(1), 0, 0, 1, 0);
+    else O::sqr(0, 0);
   }
   O::ld(a, 0);
 #pragma unroll

@@ -219,29 +219,42 @@ __device__ __forceinline__ void mont_mul_ps(uint32_t* r, const uint32_t* a, cons
 
 // Squaring, product scanning: cross products a_j a_{i-j} (j < i-j) are accumulated once and
 // doubled, the diagonal a_{i/2}^2 is added after.  N(N+1)/2 + N^2 products instead of 2 N^2.
+// The columns below N (which make m[]) and from N on (which make t[]) are two loops, as in
+// mont_mul_ps: as one loop of 2N - 1 columns nvcc does not unroll it for N = 16 and keeps m[] and t[]
+// in a local-memory frame.
 template <int N, bool FULL>
 __device__ __forceinline__ void mont_sqr_ps(uint32_t* r, const uint32_t* a) {
   uint32_t m[N], t[N];
   uint32_t u0 = 0, u1 = 0, u2 = 0, v0 = 0, v1 = 0, v2 = 0;
 #pragma unroll
-  for (int i = 0; i < 2 * N - 1; i++) {
-    const int lo = i < N ? 0 : i - N + 1;
+  for (int i = 0; i < N; i++) {
 #pragma unroll
-    for (int j = lo; 2 * j < i; j++) PBC_MAC3(u0, u1, u2, a[j], a[i - j]);
+    for (int j = 0; 2 * j < i; j++) PBC_MAC3(u0, u1, u2, a[j], a[i - j]);
 #pragma unroll
-    for (int j = lo; j <= (i < N ? i - 1 : N - 1); j++) PBC_MAC3(v0, v1, v2, m[j], c_fp.p[i - j]);
+    for (int j = 0; j < i; j++) PBC_MAC3(v0, v1, v2, m[j], c_fp.p[i - j]);
     // u = 2u (+ a_{i/2}^2), v += u
     PBC_ASM("add.cc.u32 %0, %0, %0; addc.cc.u32 %1, %1, %1; addc.u32 %2, %2, %2;"
             : "+r"(u0), "+r"(u1), "+r"(u2));
     if ((i & 1) == 0) PBC_MAC3(u0, u1, u2, a[i / 2], a[i / 2]);
     PBC_ASM("add.cc.u32 %0, %0, %3; addc.cc.u32 %1, %1, %4; addc.u32 %2, %2, %5;"
             : "+r"(v0), "+r"(v1), "+r"(v2) : "r"(u0), "r"(u1), "r"(u2));
-    if (i < N) {
-      m[i] = v0 * c_fp.np0;
-      PBC_MAC3(v0, v1, v2, m[i], c_fp.p[0]);
-    } else {
-      t[i - N] = v0;
-    }
+    m[i] = v0 * c_fp.np0;
+    PBC_MAC3(v0, v1, v2, m[i], c_fp.p[0]);
+    v0 = v1; v1 = v2; v2 = 0;
+    u0 = 0; u1 = 0; u2 = 0;
+  }
+#pragma unroll
+  for (int i = N; i < 2 * N - 1; i++) {
+#pragma unroll
+    for (int j = i - N + 1; 2 * j < i; j++) PBC_MAC3(u0, u1, u2, a[j], a[i - j]);
+#pragma unroll
+    for (int j = i - N + 1; j < N; j++) PBC_MAC3(v0, v1, v2, m[j], c_fp.p[i - j]);
+    PBC_ASM("add.cc.u32 %0, %0, %0; addc.cc.u32 %1, %1, %1; addc.u32 %2, %2, %2;"
+            : "+r"(u0), "+r"(u1), "+r"(u2));
+    if ((i & 1) == 0) PBC_MAC3(u0, u1, u2, a[i / 2], a[i / 2]);
+    PBC_ASM("add.cc.u32 %0, %0, %3; addc.cc.u32 %1, %1, %4; addc.u32 %2, %2, %5;"
+            : "+r"(v0), "+r"(v1), "+r"(v2) : "r"(u0), "r"(u1), "r"(u2));
+    t[i - N] = v0;
     v0 = v1; v1 = v2; v2 = 0;
     u0 = 0; u1 = 0; u2 = 0;
   }

@@ -1,6 +1,6 @@
 """First-light GPU probe: integer-pipe peak, F_p multiplier throughput vs occupancy, Type A
 pairing throughput (device-resident).  Prints one JSON object per line."""
-import json, os, sys, time
+import json, os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from pbc_b200.pairing import Pairing, bench_imad, kernel_launches
@@ -9,21 +9,26 @@ from pbc_b200.params import PARAMS
 def main():
     pr = Pairing(PARAMS["a"])
     sm = torch.cuda.get_device_properties(0).multi_processor_count
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "sms": sm}))
-    for blocks_per_sm, threads in ((4, 256), (8, 256), (2, 1024)):
+    smi = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "sms": sm, "power_limit_and_max_sm_clock": smi}))
+    for blocks_per_sm, threads in ((4, 256), (8, 256)):
         iters = 4000
         ms = bench_imad(sm * blocks_per_sm, threads, iters, 3)
         n = sm * blocks_per_sm * threads * 32 * iters
         print(json.dumps({"probe": "imad_wide_peak", "blocks_per_sm": blocks_per_sm, "threads": threads,
                           "ms": ms, "imad_per_s": n / (ms * 1e-3)}))
-    for mode in (0, 2, 3, 1):
-        for bps in (1, 2, 3, 4, 8):
+    # units = multiplier products (IMAD.WIDE.U32) one call executes: 528 per multiplication, 408 per squaring
+    modes = {0: ("regs_operand_scan_mul", 528), 2: ("regs_product_scan_mul", 528), 3: ("regs_sqr", 408),
+             1: ("slots_mul", 528), 6: ("slots_sqr", 408)}
+    for mode, (label, units) in modes.items():
+        for bps in (1, 2, 3, 4, 6, 8):
             iters = 2000
             ms = pr.bench_fpmul(mode, sm * bps, iters, 3)
-            muls = sm * bps * 128 * iters
-            print(json.dumps({"probe": "fpmul512", "mode": {0: "regs_operand_scan", 1: "slots_kernel_mult", 2: "regs_product_scan", 3: "regs_product_scan_sqr"}[mode], "blocks_per_sm": bps,
-                              "warps_per_sm": bps * 4, "ms": ms, "mulmod_per_s": muls / (ms * 1e-3),
-                              "imad_equiv_per_s": 528 * muls / (ms * 1e-3)}))
+            ops = sm * bps * 128 * iters
+            print(json.dumps({"probe": "fpmul512", "mode": label, "blocks_per_sm": bps, "warps_per_sm": bps * 4,
+                              "ms": ms, "ns_per_op_per_sm": ms * 1e6 * sm / ops, "ops_per_s": ops / (ms * 1e-3),
+                              "units_per_op": units, "units_per_s": units * ops / (ms * 1e-3)}))
     g = json.load(open(os.path.join(os.path.dirname(__file__), "..", "tests", "golden", "a.json")))["pairing"]
     P = b"".join(bytes.fromhex(x) for x in g["P"]); Q = b"".join(bytes.fromhex(x) for x in g["Q"])
     m = len(g["e"])

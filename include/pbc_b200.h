@@ -192,7 +192,9 @@ const char *pbc_b200_last_error(void);
  *          base-field prime; mode 0 = operand-scanning multiplier in registers, 1 = the multiplier
  *          the kernels use, through the shared-memory slot machine, 2 = product-scanning
  *          multiplier in registers, 3 = the squaring the kernels use, in registers, 6 (type a) = that
- *          squaring through the slot machine.  muls = threads * iters.
+ *          squaring through the slot machine, 7 (type a) = the lazy two-product routine of the Miller
+ *          step through the slot machine (two products, one reduction: about 1.5 multiplications'
+ *          work).  muls = threads * iters.
  *   imad : IMAD.WIDE.U32 issue-rate probe, 32 * iters instructions per thread: the faster of two
  *          kernels, four independent carry chains of eight and eight carry-free chains of four
  *          (data-dependent multiplicands in both).

@@ -72,9 +72,10 @@ __global__ void k_fpmul_chain(uint32_t* __restrict__ out, const uint32_t* __rest
 
 // Same chain through the shared-memory slot machine (what the pairing kernels execute).
 // MIX 0: multiplications only; 1: one multiplication + one addition per step as separate calls (the
-// Miller loop's mix is 19 : 22); 2: the same work as one fused call; 3: squarings only (O::sqr).
+// Miller loop's mix is 19 : 22); 2: the same work as one fused call; 3: squarings only (O::sqr);
+// 4: the lazy two-product routine of the type A Miller step (O::lazy: 2 x 256 products + one 272-unit reduction).
 template <int N, bool FULL, int BLOCK, int MIX>
-__global__ void __launch_bounds__(BLOCK)
+__global__ void __launch_bounds__(BLOCK, MIX == 4 ? 3 : 1)
 k_fpmul_slots(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int iters) {
   using O = Ops<N, FULL, BLOCK>;
   size_t T = (size_t)gridDim.x * BLOCK, t = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -86,6 +87,7 @@ k_fpmul_slots(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int i
     if (MIX == 0) O::mul(0, 0, 1);
     else if (MIX == 1) { O::mul(0, 0, 1); O::add(0, 0, 1); }
     else if (MIX == 2) O::fmul(0, 0, 1, O::F_ADD_C1(1), 0, 0, 1, 0);
+    else if (MIX == 4) O::lazy(0, O::LZ_TWO, 0, 1, 1, 0, 0, 0, nullptr, 0);   // (a b + b a) / R: two products, one reduction
     else O::sqr(0, 0);
   }
   O::ld(a, 0);

@@ -1529,6 +1529,7 @@ static double bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters
       else if (mode == 4) k_fpmul_slots<kNA, true, 128, 1><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else if (mode == 5) k_fpmul_slots<kNA, true, 128, 2><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else if (mode == 6) k_fpmul_slots<kNA, true, 128, 3><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
+      else if (mode == 7) k_fpmul_slots<kNA, true, 128, 4><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else k_fpmul_slots<kNA, true, 128, 0><<<blocks, threads, smem, st>>>(out, in, iters);
     } else {
       k_fqmul_chain<<<blocks, threads, 0, st>>>(out, in, iters, mode == 3 ? 1 : 0);

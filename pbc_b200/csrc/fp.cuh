@@ -162,6 +162,155 @@ __device__ __forceinline__ void mont_mul(uint32_t* r, const uint32_t* a, const u
 }
 
 // ---------------------------------------------------------------------------------------------
+// Double width: lazy reduction.  A sum of products is accumulated unreduced in 2N + 1 words and
+// reduced once, so each product after the first costs N^2 IMAD.WIDE instead of N^2 + N^2 + N.
+// The caller keeps the value handed to redc_wide in [0, 2 q R) (q < R = 2^(32N) for any q):
+//   a b + c d < 2 q^2,  a b - c d + q R < q^2 + q R,  and a stored S' < q R in  a b - S' + q R.
+// Intermediate values may be negative: the 2N + 1 words are exact modulo 2^(32(2N+1)).
+// ---------------------------------------------------------------------------------------------
+// One row of the plain product: mont_round without the m p half.  w[0] on exit is a finished
+// column.  The running sum a (b mod 2^(32(i+1))) / 2^(32i) stays below 2^(32(N+1)): no top word.
+template <int N>
+__device__ __forceinline__ void wide_round(uint32_t* z, uint32_t* w, const uint32_t* a, uint32_t bi, bool first) {
+  if (first) {
+    chain_mul<N>(z, a + 1, bi);
+    chain_mul<N>(w, a, bi);
+  } else {
+    PBC_ASM("add.cc.u32 %0, %0, %1;" : "+r"(w[0]) : "r"(z[1]));
+    chain_mad_shift<N>(z, a + 1, bi, 0);
+    chain_mad<N>(w, a, bi);
+    PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(z[N - 1]));
+  }
+}
+
+// p[0..2N) = a*b, operand scanning on the even / odd accumulators: one IMAD.WIDE per product.
+template <int N>
+__device__ __forceinline__ void mul_wide(uint32_t* p, const uint32_t* a, const uint32_t* b) {
+  static_assert(N % 2 == 0, "even limb count");
+  uint32_t x[N], y[N];
+  wide_round<N>(x, y, a, b[0], true);
+  p[0] = y[0];
+#pragma unroll
+  for (int i = 1; i < N; i += 2) {
+    wide_round<N>(y, x, a, b[i], false);
+    p[i] = x[0];
+    if (i + 1 < N) {
+      wide_round<N>(x, y, a, b[i + 1], false);
+      p[i + 1] = y[0];
+    }
+  }
+  // the last row ran as (y, x): the high half is (x >> 32) + y
+  PBC_ASM("add.cc.u32 %0, %1, %2;" : "=r"(p[N]) : "r"(x[1]), "r"(y[0]));
+#pragma unroll
+  for (int k = 1; k < N - 1; k++)
+    PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(p[N + k]) : "r"(x[k + 1]), "r"(y[k]));
+  PBC_ASM("addc.u32 %0, %1, 0;" : "=r"(p[2 * N - 1]) : "r"(y[N - 1]));
+}
+
+// acc[0..2N] += p[0..2N)
+template <int N>
+__device__ __forceinline__ void wide_add(uint32_t* acc, const uint32_t* p) {
+  PBC_ASM("add.cc.u32 %0, %0, %1;" : "+r"(acc[0]) : "r"(p[0]));
+#pragma unroll
+  for (int k = 1; k < 2 * N; k++) PBC_ASM("addc.cc.u32 %0, %0, %1;" : "+r"(acc[k]) : "r"(p[k]));
+  PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(acc[2 * N]));
+}
+
+// acc[0..2N] -= p[0..2N)
+template <int N>
+__device__ __forceinline__ void wide_sub(uint32_t* acc, const uint32_t* p) {
+  PBC_ASM("sub.cc.u32 %0, %0, %1;" : "+r"(acc[0]) : "r"(p[0]));
+#pragma unroll
+  for (int k = 1; k < 2 * N; k++) PBC_ASM("subc.cc.u32 %0, %0, %1;" : "+r"(acc[k]) : "r"(p[k]));
+  PBC_ASM("subc.u32 %0, %0, 0;" : "+r"(acc[2 * N]));
+}
+
+// acc[0..2N] += p R
+template <int N>
+__device__ __forceinline__ void wide_add_pR(uint32_t* acc) {
+  PBC_ASM("add.cc.u32 %0, %0, %1;" : "+r"(acc[N]) : "r"(c_fp.p[0]));
+#pragma unroll
+  for (int k = 1; k < N; k++) PBC_ASM("addc.cc.u32 %0, %0, %1;" : "+r"(acc[N + k]) : "r"(c_fp.p[k]));
+  PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(acc[2 * N]));
+}
+
+// acc[0..2N] -= p R if acc >= p R.  For 0 <= acc < 2 p R the result is below p R (acc[2N] = 0).
+template <int N>
+__device__ __forceinline__ void wide_sub_pR_if_ge(uint32_t* acc) {
+  uint32_t d[N + 1], borrow;
+  PBC_ASM("sub.cc.u32 %0, %1, %2;" : "=r"(d[0]) : "r"(acc[N]), "r"(c_fp.p[0]));
+#pragma unroll
+  for (int k = 1; k < N; k++) PBC_ASM("subc.cc.u32 %0, %1, %2;" : "=r"(d[k]) : "r"(acc[N + k]), "r"(c_fp.p[k]));
+  PBC_ASM("subc.cc.u32 %0, %1, 0;" : "=r"(d[N]) : "r"(acc[2 * N]));
+  PBC_ASM("subc.u32 %0, 0, 0;" : "=r"(borrow));   // 0 if acc >= p R
+#pragma unroll
+  for (int k = 0; k <= N; k++) acc[N + k] = borrow ? acc[N + k] : d[k];
+}
+
+// One row of the Montgomery reduction of a stored value: mont_round without the a b_i half.  The
+// running sum starts as the low N words of t; the shift by one word rides on the odd-aligned chain.
+template <int N>
+__device__ __forceinline__ void redc_round(uint32_t* z, uint32_t* w, uint32_t& top, bool first) {
+  uint32_t m;
+  if (first) {
+    m = w[0] * c_fp.np0;
+    chain_mul<N>(z, c_fp.p + 1, m);
+    top = 0;
+  } else {
+    // w[0] + z[1] is column 0; its carry enters the shifting chain at column 1
+    PBC_ASM("add.cc.u32 %0, %0, %2; mul.lo.u32 %1, %0, %3;" : "+r"(w[0]), "=r"(m) : "r"(z[1]), "r"(c_fp.np0));
+    chain_mad_shift<N>(z, c_fp.p + 1, m, top);
+    top = carry_out();
+  }
+  chain_mad<N>(w, c_fp.p, m);
+  PBC_ASM("addc.cc.u32 %0, %0, 0;" : "+r"(z[N - 1]));
+  PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(top));
+}
+
+// r = t / R mod p, fully reduced, for 0 <= t < 2 p R (t[0..2N], t[2N] the top word).
+// (t_lo + M p) / R <= p is formed on the even / odd accumulators (N^2 IMAD.WIDE + N IMAD), t_hi < 2p is
+// added, and the sum (< 3p) takes up to two conditional subtractions of p.
+template <int N>
+__device__ __forceinline__ void redc_wide(uint32_t* r, const uint32_t* t) {
+  static_assert(N % 2 == 0, "even limb count");
+  uint32_t x[N], y[N], top;
+#pragma unroll
+  for (int k = 0; k < N; k++) y[k] = t[k];
+  redc_round<N>(x, y, top, true);
+#pragma unroll
+  for (int i = 1; i < N; i += 2) {
+    redc_round<N>(y, x, top, false);
+    if (i + 1 < N) redc_round<N>(x, y, top, false);
+  }
+  // s = (x >> 32) + y + top 2^(32N) + t_hi
+  uint32_t s[N];
+  PBC_ASM("add.cc.u32 %0, %1, %2;" : "=r"(s[0]) : "r"(x[1]), "r"(y[0]));
+#pragma unroll
+  for (int k = 1; k < N - 1; k++) PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(s[k]) : "r"(x[k + 1]), "r"(y[k]));
+  PBC_ASM("addc.cc.u32 %0, %1, 0;" : "=r"(s[N - 1]) : "r"(y[N - 1]));
+  PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(top));
+  PBC_ASM("add.cc.u32 %0, %0, %1;" : "+r"(s[0]) : "r"(t[N]));
+#pragma unroll
+  for (int k = 1; k < N; k++) PBC_ASM("addc.cc.u32 %0, %0, %1;" : "+r"(s[k]) : "r"(t[N + k]));
+  PBC_ASM("addc.u32 %0, %0, %1;" : "+r"(top) : "r"(t[2 * N]));
+#pragma unroll
+  for (int pass = 0; pass < 2; pass++) {
+    uint32_t d[N], dtop;
+    PBC_ASM("sub.cc.u32 %0, %1, %2;" : "=r"(d[0]) : "r"(s[0]), "r"(c_fp.p[0]));
+#pragma unroll
+    for (int k = 1; k < N; k++) PBC_ASM("subc.cc.u32 %0, %1, %2;" : "=r"(d[k]) : "r"(s[k]), "r"(c_fp.p[k]));
+    PBC_ASM("subc.cc.u32 %0, %1, 0;" : "=r"(dtop) : "r"(top));
+    uint32_t borrow;
+    PBC_ASM("subc.u32 %0, 0, 0;" : "=r"(borrow));   // 0 if s >= p
+#pragma unroll
+    for (int k = 0; k < N; k++) s[k] = borrow ? s[k] : d[k];
+    top = borrow ? top : dtop;
+  }
+#pragma unroll
+  for (int k = 0; k < N; k++) r[k] = s[k];
+}
+
+// ---------------------------------------------------------------------------------------------
 // Product-scanning (column-wise) variant.  Every 32x32 product is one IMAD.WIDE.U32 with
 // carry-OUT only (no carry-in: the .X form may issue at a lower rate), the carry
 // is absorbed by an IADD3.X on the ALU pipe, so the FMA and ALU pipes alternate.  Two

@@ -269,7 +269,10 @@ enum A9Slot { nX, nY, nZ, nF0, nF1, nT0, nT1, nT2, nT3, kA9Slots };
 
 // qx, qy: this thread's Q coordinates in the global array (Montgomery form), vectors n apart.
 // a_step_9_line: on entry g = (nT0, nF1) and the f0 slot is free; on exit f' = g l in (nF0, nF1), V doubled.
-template <class O>
+// LAZY: Re l and f' take one Montgomery reduction per sum of products (Ops::lazy), 544 of the step's 8 256
+// multiplier units fewer.  Ops::lazy needs about 130 registers; k_a_miller9 fits it in 168 (three blocks
+// per SM), k_a_miller9_shared keeps more live across its calls and does not, so it runs LAZY = false.
+template <class O, bool LAZY>
 __device__ __forceinline__ void a_step_9_line(const uint4* qx, const uint4* qy, size_t n) {
   O::sqr(nT1, nX);                                   // A
   O::sqr(nT2, nY);                                   // B
@@ -278,10 +281,14 @@ __device__ __forceinline__ void a_step_9_line(const uint4* qx, const uint4* qy, 
   O::add(nT3, nT1, nT3);                             // A' = A + C
   O::dbl(nT1, nT3);
   O::add(nT1, nT1, nF0);                             // U = 3A + C
-  O::mulp(nT1, nT1, nZ);
-  O::mulg(nT1, nT1, qx, n);                          // U Z Qx
-  O::mulp(nX, nX, nF0);                              // X T
-  O::add(nT1, nT1, nX);                              // Re l                   (X slot is free)
+  O::mulp(nT1, nT1, nZ);                             // U Z
+  if constexpr (LAZY) {
+    O::lazy(nT1, O::LZ_TWO | O::LZ_GLOBAL_B, nT1, 0, nX, nF0, 0, 0, qx, n);   // Re l = U Z Qx + X T, one reduction
+  } else {
+    O::mulg(nT1, nT1, qx, n);                        // U Z Qx
+    O::mulp(nX, nX, nF0);                            // X T
+    O::add(nT1, nT1, nX);                            // Re l                   (X slot is free)
+  }
   O::sqr(nX, nF0);                                   // X' = T^2
   O::sqr(nT3, nT3);
   O::dbl(nT3, nT3);
@@ -294,13 +301,20 @@ __device__ __forceinline__ void a_step_9_line(const uint4* qx, const uint4* qy, 
   O::mulp(nF0, nY, nZ);
   O::dbl(nF0, nF0);
   O::mulg(nF0, nF0, qy, n);                          // Im l = 2 Y Z Qy
-  O::dbl(nZ, nT2, 2);                                // Z' = 4 B
-  O::template mul2<false>(nT2, nT0, nF1, nT1, nF0);  // (g0 + g1)(Re l + Im l)
-  O::mulp(nT0, nT0, nT1);                            // g0 Re l
-  O::mulp(nF1, nF1, nF0);                            // g1 Im l
-  O::sub(nF0, nT0, nF1);                             // f0'
-  O::sub(nT2, nT2, nT0);
-  O::sub(nF1, nT2, nF1);                             // f1'
+  O::dbl(nZ, nT2, 2);                                // Z' = 4 B                (B and Y are dead)
+  if constexpr (LAZY) {
+    // f' = g l with unreduced products P1 = g0 Re l, P2 = g1 Im l:  f0' = (P1 - P2 + q R) / R,
+    // S' = P1 + P2 (- q R) into (nT2, nY), g0 + g1 into nT0, Re l + Im l into nT1
+    O::lazy(nF0, O::LZ_TWO | O::LZ_SUB | O::LZ_ADD_QR | O::LZ_KARATSUBA, nT0, nT1, nF1, nF0, nT2, nY, nullptr, 0);
+    O::lazy(nF1, O::LZ_SUB_S | O::LZ_ADD_QR, nT0, nT1, 0, 0, nT2, nY, nullptr, 0);   // f1' = ((g0 + g1)(Re l + Im l) - S' + q R) / R
+  } else {
+    O::template mul2<false>(nT2, nT0, nF1, nT1, nF0);  // (g0 + g1)(Re l + Im l)
+    O::mulp(nT0, nT0, nT1);                            // g0 Re l
+    O::mulp(nF1, nF1, nF0);                            // g1 Im l
+    O::sub(nF0, nT0, nF1);                             // f0'
+    O::sub(nT2, nT2, nT0);
+    O::sub(nF1, nT2, nF1);                             // f1'
+  }
   O::copy(nY, nT3);
 }
 // g = f^2 into (nT0, nF1): g0 = (f0 + f1)(f0 - f1), g1 = 2 f0 f1   (the f0 slot is free afterwards)
@@ -313,7 +327,7 @@ __device__ __forceinline__ void a_step_9_square() {
 template <class O>
 __device__ __forceinline__ void a_double_step_9(const uint4* qx, const uint4* qy, size_t n) {
   a_step_9_square<O>();
-  a_step_9_line<O>(qx, qy, n);
+  a_step_9_line<O, true>(qx, qy, n);
 }
 
 // f *= (l0 + i l1) with two temporaries (t0, t1); l0, l1 are preserved
@@ -635,7 +649,7 @@ k_a_miller9_shared(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q,
         O::st_global(save, 1, np, pr, nF0);
         O::st_global(save, 2, np, pr, nZ);
       }
-      a_step_9_line<O>(qm + pr, qm + 4 * np + pr, np);
+      a_step_9_line<O, false>(qm + pr, qm + 4 * np + pr, np);
       if (live) {
         O::st_global(vj, 0, np, pr, nX);
         O::st_global(vj, 1, np, pr, nY);

@@ -74,27 +74,28 @@ struct Ops {
   // variant: with 12 warps per SM the four separate copies (mul, mul2<+>, mul2<->, mulg: 3 200
   // instructions, 51 KB) made instruction fetch a leading stall.
   static constexpr uint32_t MX_ADD_A = 1u, MX_ADD_B = 2u, MX_SUB_B = 4u, MX_GLOBAL_B = 8u;
-  static __device__ __noinline__ void mulx(int d, int a, int b, uint32_t mode, int a2, int b2, const void* g, size_t n) {
-    uint32_t x[N], y[N];
-    if (mode & MX_GLOBAL_B) {
-      if constexpr (kVecWords == 4) {
-        const uint4* p = reinterpret_cast<const uint4*>(g);
+  // r = the element at g (limb-major global array, vectors n apart)
+  static __device__ __forceinline__ void ld_g(uint32_t* r, const void* g, size_t n) {
+    if constexpr (kVecWords == 4) {
+      const uint4* p = reinterpret_cast<const uint4*>(g);
 #pragma unroll
-        for (int v = 0; v < kVecs; v++) {
-          uint4 q = p[v * n];
-          y[4 * v] = q.x; y[4 * v + 1] = q.y; y[4 * v + 2] = q.z; y[4 * v + 3] = q.w;
-        }
-      } else {
-        const uint2* p = reinterpret_cast<const uint2*>(g);
-#pragma unroll
-        for (int v = 0; v < kVecs; v++) {
-          uint2 q = p[v * n];
-          y[2 * v] = q.x; y[2 * v + 1] = q.y;
-        }
+      for (int v = 0; v < kVecs; v++) {
+        uint4 q = p[v * n];
+        r[4 * v] = q.x; r[4 * v + 1] = q.y; r[4 * v + 2] = q.z; r[4 * v + 3] = q.w;
       }
     } else {
-      ld(y, b);
+      const uint2* p = reinterpret_cast<const uint2*>(g);
+#pragma unroll
+      for (int v = 0; v < kVecs; v++) {
+        uint2 q = p[v * n];
+        r[2 * v] = q.x; r[2 * v + 1] = q.y;
+      }
     }
+  }
+  static __device__ __noinline__ void mulx(int d, int a, int b, uint32_t mode, int a2, int b2, const void* g, size_t n) {
+    uint32_t x[N], y[N];
+    if (mode & MX_GLOBAL_B) ld_g(y, g, n);
+    else ld(y, b);
     if (mode & (MX_ADD_B | MX_SUB_B)) {
       ld(x, b2);
       if (mode & MX_ADD_B) fp_add<N, FULL>(y, y, x); else fp_sub<N>(y, y, x);
@@ -116,6 +117,63 @@ struct Ops {
     mulx(d, a, 0, MX_GLOBAL_B, 0, 0, g, n);
   }
   static __device__ __forceinline__ void mulp(int d, int a, int b) { mulx(d, a, b, 0, 0, 0, nullptr, 0); }
+
+  // ---- lazy reduction (fp.cuh mul_wide / redc_wide; FULL, even N) ----
+  //   d = (a0 b0 [+- a1 b1] [+ q R] [- S]) / R mod q,   S = the unreduced value in slots (s0, s1)
+  // One Montgomery reduction for the whole sum: a second product costs N^2 IMAD.WIDE, not N^2 + N^2 + N.
+  // LZ_GLOBAL_B: b0 is the element at g (as in mulx).  LZ_KARATSUBA (with LZ_TWO): also stores
+  // S' = a0 b0 + a1 b1, less q R if that is >= q R, into (s0, s1), a0 + a1 into a0 and b0 + b1 into b0.
+  // The caller keeps the sum in [0, 2 q R).  One 256-product body and one reduction body: the terms
+  // are a loop, not unrolled.  d may alias any operand slot (everything is read before d is written).
+  static constexpr uint32_t LZ_TWO = 1u, LZ_SUB = 2u, LZ_ADD_QR = 4u, LZ_SUB_S = 8u, LZ_GLOBAL_B = 16u,
+                            LZ_KARATSUBA = 32u;
+  static __device__ __noinline__ void lazy(int d, uint32_t mode, int a0, int b0, int a1, int b1, int s0, int s1,
+                                           const void* g, size_t n) {
+    static_assert(FULL && N % 2 == 0, "lazy reduction: 512-bit field");
+    uint32_t acc[2 * N + 1];
+    if (mode & LZ_SUB_S) {
+      uint32_t z[2 * N];
+      ld(z, s0); ld(z + N, s1);
+#pragma unroll
+      for (int k = 0; k <= 2 * N; k++) acc[k] = 0;
+      wide_sub<N>(acc, z);
+    } else {
+#pragma unroll
+      for (int k = 0; k <= 2 * N; k++) acc[k] = 0;
+    }
+    const int terms = (mode & LZ_TWO) ? 2 : 1;
+#pragma unroll 1
+    for (int t = 0; t < terms; t++) {
+      uint32_t x[N], y[N], p[2 * N];
+      if (t == 0 && (mode & LZ_GLOBAL_B)) ld_g(y, g, n);
+      else ld(y, t ? b1 : b0);
+      ld(x, t ? a1 : a0);
+      mul_wide<N>(p, x, y);
+      if (t == 1 && (mode & LZ_KARATSUBA)) {
+        uint32_t s[2 * N + 1];
+#pragma unroll
+        for (int k = 0; k <= 2 * N; k++) s[k] = acc[k];
+        wide_add<N>(s, p);
+        wide_sub_pR_if_ge<N>(s);
+        st(s0, s); st(s1, s + N);
+      }
+      if (t == 1 && (mode & LZ_SUB)) wide_sub<N>(acc, p);
+      else wide_add<N>(acc, p);
+    }
+    if (mode & LZ_ADD_QR) wide_add_pR<N>(acc);
+    if (mode & LZ_KARATSUBA) {
+      uint32_t x[N], y[N];
+      ld(x, a0); ld(y, a1);
+      fp_add<N, FULL>(x, x, y);
+      st(a0, x);
+      ld(x, b0); ld(y, b1);
+      fp_add<N, FULL>(x, x, y);
+      st(b0, x);
+    }
+    uint32_t r[N];
+    redc_wide<N>(r, acc);
+    st(d, r);
+  }
   // d = a*b - c
   static __device__ __noinline__ void mulsub(int d, int a, int b, int c) {
     uint32_t x[N], y[N];

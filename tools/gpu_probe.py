@@ -18,9 +18,10 @@ def main():
         n = sm * blocks_per_sm * threads * 32 * iters
         print(json.dumps({"probe": "imad_wide_peak", "blocks_per_sm": blocks_per_sm, "threads": threads,
                           "ms": ms, "imad_per_s": n / (ms * 1e-3)}))
-    # units = multiplier products (IMAD.WIDE.U32) one call executes: 528 per multiplication, 408 per squaring
+    # units = multiplier products (IMAD.WIDE.U32) one call executes: 528 per multiplication, 408 per squaring,
+    # 2 x 256 + 272 = 784 for the lazy two-product routine (two products, one reduction)
     modes = {0: ("regs_operand_scan_mul", 528), 2: ("regs_product_scan_mul", 528), 3: ("regs_sqr", 408),
-             1: ("slots_mul", 528), 6: ("slots_sqr", 408)}
+             1: ("slots_mul", 528), 6: ("slots_sqr", 408), 7: ("slots_lazy_two_products", 784)}
     for mode, (label, units) in modes.items():
         for bps in (1, 2, 3, 4, 6, 8):
             iters = 2000

@@ -71,9 +71,8 @@ __global__ void k_fpmul_chain(uint32_t* __restrict__ out, const uint32_t* __rest
 }
 
 // Same chain through the shared-memory slot machine (what the pairing kernels execute).
-// MIX 0: multiplications only; 1: one multiplication + one addition per step as separate calls (the
-// Miller loop's mix is 19 : 22); 2: the same work as one fused call; 3: squarings only (O::sqr);
-// 4: the lazy two-product routine of the type A Miller step (O::lazy: 2 x 256 products + one 272-unit reduction).
+// MIX 0: multiplications only; 3: squarings only (O::sqr); 4: the lazy two-product routine of the
+// type A Miller step (O::lazy: 2 x 256 products + one 272-unit reduction).
 template <int N, bool FULL, int BLOCK, int MIX>
 __global__ void __launch_bounds__(BLOCK, MIX == 4 ? 3 : 1)
 k_fpmul_slots(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int iters) {
@@ -85,8 +84,6 @@ k_fpmul_slots(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int i
   O::st(0, a); O::st(1, b);
   for (int i = 0; i < iters; i++) {
     if (MIX == 0) O::mul(0, 0, 1);
-    else if (MIX == 1) { O::mul(0, 0, 1); O::add(0, 0, 1); }
-    else if (MIX == 2) O::fmul(0, 0, 1, O::F_ADD_C1(1), 0, 0, 1, 0);
     else if (MIX == 4) O::lazy(0, O::LZ_TWO, 0, 1, 1, 0, 0, 0, nullptr, 0);   // (a b + b a) / R: two products, one reduction
     else O::sqr(0, 0);
   }

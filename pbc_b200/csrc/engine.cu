@@ -27,7 +27,6 @@
 #include "pairing_d.cuh"
 #include "pairing_f.cuh"
 #include "pairing_f_slots.cuh"
-#include "pairing_f_pair.cuh"
 #include "pairing_g.cuh"
 #include "group_a.cuh"
 #include "group_a1.cuh"
@@ -190,20 +189,6 @@ struct Job {
 
 static size_t cc_table_bytes(const pbc_b200_pairing_s* p);
 
-// PBC_A_SLOTS: slots of the type A Miller kernel of pairings and unshared products.  9 (default):
-// k_a_miller9, three 128-thread blocks per SM; 7: k_a_miller7, four blocks -- 2.5 % fewer cycles per
-// pairing, but on a power-capped H100 the clock drops more than that (DESIGN.md 3.8); 14: k_a_miller of
-// round 1, two blocks.  7 and 14 are kept for A/B runs.  Products that share an accumulator run
-// k_a_miller9_shared in every setting.
-#ifndef PBC_A_SLOTS
-#define PBC_A_SLOTS 9
-#endif
-static_assert(PBC_A_SLOTS == 7 || PBC_A_SLOTS == 9 || PBC_A_SLOTS == 14, "PBC_A_SLOTS: 7, 9 or 14");
-// threads of the type A Miller grid for n pairings (whole blocks)
-static size_t a_miller_cols(size_t n) { return (n + kBlockMiller - 1) / kBlockMiller * kBlockMiller; }
-// the g array of k_a_miller7 (f^2 and g0 + g1, one column per thread of its grid); the other kernels need none
-static size_t a_miller_g_bytes(size_t n) { return PBC_A_SLOTS == 7 ? 3 * 64 * a_miller_cols(n) : 0; }
-
 // workspace bytes for n_out outputs of `job`
 static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out) {
   if (p->type == '1') {
@@ -215,12 +200,11 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
   }
   if (p->type == 'a') {
     const size_t fq = 64;
-    // f [2], dprod, prefix, save [5] (V1, f1), qm [2] (Montgomery-form Q of the nine- and seven-slot
-    // Miller kernels), then the g array of the seven-slot kernel
-    if (job.mode == kSingle) return n_out * (2 + 1 + 1 + 5 + 2) * fq + a_miller_g_bytes(n_out);
+    // f [2], dprod, prefix, save [5] (V1, f1), qm [2] (Montgomery-form Q of the Miller kernels)
+    if (job.mode == kSingle) return n_out * (2 + 1 + 1 + 5 + 2) * fq;
     // products: + vj [3] per pair (V of the pairs that share an accumulator, k_a_miller9_shared)
     if (job.mode == kProd)
-      return n_out * job.k * (2 + 1 + 5 + 2 + 3) * fq + n_out * (2 + 1 + 1) * fq + a_miller_g_bytes(n_out * job.k);
+      return n_out * job.k * (2 + 1 + 5 + 2 + 3) * fq + n_out * (2 + 1 + 1) * fq;
     return n_out * (2 + 1 + 1) * fq + (size_t)(3 * (p->a.exp2 + 1) * kNA + 4) * 4;
   }
   // types f, d: Miller values [W][n] words + one flag word each; products add the reduced arrays
@@ -790,32 +774,13 @@ static cudaError_t allow_smem(K kernel, size_t bytes) {
   return cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
 }
 
-static constexpr size_t kSmemAMiller = (size_t)kASlots * 64 * kBlockMiller;
 static constexpr size_t kSmemAMiller9 = (size_t)kA9Slots * 64 * kBlockMiller;
-static constexpr size_t kSmemAMiller7 = (size_t)kA7Slots * 64 * kBlockMiller;
 // PBC_F_SLOTS = 1 (default): type F Miller loop on the shared-memory slot machine (pairing_f_slots.cuh)
 // where the parameters allow it; 0: the round-1 kernel (local-memory frames)
 #ifndef PBC_F_SLOTS
 #define PBC_F_SLOTS 1
 #endif
 static constexpr int kBlockFS = 128;
-// PBC_F_PAIR = 1: the type F Miller loop with two lanes per pairing (pairing_f_pair.cuh): k_f_prep + k_f_miller_p.
-// Bit-exact (simulator test + GPU fixtures) and no faster than k_f_miller_s: sixteen resident warps instead of eight
-// leave the multiplier pipe as busy as before, so latency is not what holds the slot kernel back.  Kept off.
-#ifndef PBC_F_PAIR
-#define PBC_F_PAIR 0
-#endif
-#ifndef PBC_FP_PAIRS
-#define PBC_FP_PAIRS 128
-#endif
-static constexpr int kPairsFP = PBC_FP_PAIRS;    // pairings per block (twice as many threads)
-static constexpr size_t kSmemFMillerP = (size_t)kFPSlots * kNS * 4 * kPairsFP;
-// the CPU simulator (tests/host) runs the two lanes of a pair on two host threads when told to
-#ifdef PBC_HOST_SIM
-#define PBC_PAIR_LAUNCH(on) (::cusim::pair_mode() = (on))
-#else
-#define PBC_PAIR_LAUNCH(on) ((void)0)
-#endif
 // threads per block of the slot-machine Miller kernel: 128 -> two blocks (8 warps) per SM, 96 -> three blocks (9 warps)
 #ifndef PBC_FS_MILLER_BLOCK
 #define PBC_FS_MILLER_BLOCK 128
@@ -854,9 +819,7 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
     CUDA_OK(cudaDeviceGetAttribute(&c.sms, cudaDevAttrMultiProcessorCount, dev));
     for (int s = 0; s < 2; s++) CUDA_OK(cudaStreamCreateWithFlags(&c.stream[s], cudaStreamNonBlocking));
     if (p->type == 'a') {
-      CUDA_OK(allow_smem(k_a_miller<kBlockMiller>, kSmemAMiller));
       CUDA_OK(allow_smem(k_a_miller9<kBlockMiller>, kSmemAMiller9));
-      CUDA_OK(allow_smem(k_a_miller7<kBlockMiller>, kSmemAMiller7));
       CUDA_OK(allow_smem(k_a_miller9_shared<kBlockMiller>, kSmemAMiller9));
       CUDA_OK(allow_smem(k_a_finalexp<kBlockFinal>, kSmemAFinal));
       CUDA_OK(allow_smem(k_batch_invert<kNA, true, kBlockInv>, kSmemInv16));
@@ -872,7 +835,6 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
       CUDA_OK(allow_smem(k_a_g1_decompress<kBlockMiller>, (size_t)5 * 64 * kBlockMiller));
     }
     if (p->type == 'f') CUDA_OK(allow_smem(k_f_miller_s<kBlockFSM>, kSmemFMillerS));
-    if (p->type == 'f') CUDA_OK(allow_smem(k_f_miller_p<kPairsFP>, kSmemFMillerP));
     if (p->type == 'f') CUDA_OK(allow_smem(k_f_finalexp_s<kBlockFS>, kSmemFFinalS));
     if (p->type == '1') {
       CUDA_OK(allow_smem(k_a1_miller<kBlockA1>, kSmemA1Miller));
@@ -967,15 +929,6 @@ static size_t inv_threads(const pbc_b200_pairing_s* p, size_t n, size_t per_sm) 
   return n < t ? n : t;
 }
 
-// the type A Miller kernel PBC_A_SLOTS selects, one thread per pairing; g: [3][4][a_miller_cols(n)] uint4
-static void launch_a_miller(const uint8_t* P, const uint8_t* Q, uint4* f, uint4* dprod, uint4* save, uint4* qm,
-                            uint4* g, size_t n, cudaStream_t st) {
-  unsigned gm = (unsigned)(a_miller_cols(n) / kBlockMiller);
-  if (PBC_A_SLOTS == 7) k_a_miller7<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller7, st>>>(P, Q, f, dprod, save, qm, g, n);
-  else if (PBC_A_SLOTS == 9) k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(P, Q, f, dprod, save, qm, n);
-  else k_a_miller<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller, st>>>(P, Q, f, dprod, save, n);
-}
-
 // ------------------------------------------------------------------------------------------
 // enqueue one batch of n_out outputs of `job`, device buffers, on `st`.  ws: ws_bytes() bytes.
 // ------------------------------------------------------------------------------------------
@@ -1045,8 +998,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       prefix = dprod + 4 * n;                    // [4][n]
       uint4* save = prefix + 4 * n;              // [5][4][n]
       uint4* qm = save + 20 * n;                 // [2][4][n]
-      uint4* g = qm + 8 * n;                     // a_miller_g_bytes(n)
-      launch_a_miller(d_in1, d_in2, f, dprod, save, qm, g, n, st);
+      unsigned gm = (unsigned)((n + kBlockMiller - 1) / kBlockMiller);
+      k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, f, dprod, save, qm, n);
       LAUNCHED();
     } else if (job.mode == kProd) {
       size_t m = n * job.k;
@@ -1058,16 +1011,13 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       f = vj + 12 * m;                           // [2][4][n]
       dprod = f + 8 * n;
       prefix = dprod + 4 * n;
-      uint4* g = prefix + 4 * n;                 // a_miller_g_bytes(m)
       // pairs per thread sharing one accumulator: the largest divisor of k not above the handle's setting
       // that still leaves four waves of threads (sharing divides the thread count, and with too few
       // threads the GPU idles)
       size_t share = 1;
-      if (PBC_A_SLOTS != 14) {
-        const size_t wave = cur_sms(p) * 3 * kBlockMiller;
-        for (size_t c = (size_t)p->prod_share; c > 1; c--)
-          if (job.k % c == 0 && (m / c >= 4 * wave || p->prod_share_forced)) { share = c; break; }
-      }
+      const size_t wave = cur_sms(p) * 3 * kBlockMiller;
+      for (size_t c = (size_t)p->prod_share; c > 1; c--)
+        if (job.k % c == 0 && (m / c >= 4 * wave || p->prod_share_forced)) { share = c; break; }
       size_t kk = job.k, mm = m;                 // pairs per output / Miller values that reach k_a_prod
       if (share > 1) {
         mm = m / share;
@@ -1075,7 +1025,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
         unsigned gs = (unsigned)((mm + kBlockMiller - 1) / kBlockMiller);
         k_a_miller9_shared<kBlockMiller><<<gs, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, fi, di, save, qm, vj, mm, share);
       } else {
-        launch_a_miller(d_in1, d_in2, fi, di, save, qm, g, m, st);
+        unsigned gm = (unsigned)((m + kBlockMiller - 1) / kBlockMiller);
+        k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, fi, di, save, qm, m);
       }
       LAUNCHED();
       unsigned gp = (unsigned)((n + kBlockProd - 1) / kBlockProd);
@@ -1131,13 +1082,6 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     }
     if (isf && PBC_F_SLOTS && p->f.slots_ok) {
       uint32_t* gq = mv + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0);   // after the Miller values and flags
-      if (PBC_F_PAIR) {
-        k_f_prep<kBlockCC><<<(unsigned)((m + kBlockCC - 1) / kBlockCC), kBlockCC, 0, st>>>(d_in1, d_in2, flag, gq, m, stride1, tab, rows);
-        LAUNCHED();
-        PBC_PAIR_LAUNCH(true);
-        k_f_miller_p<kPairsFP><<<(unsigned)((m + kPairsFP - 1) / kPairsFP), 2 * kPairsFP, kSmemFMillerP, st>>>(mv, flag, gq, m, tab, rows);
-        PBC_PAIR_LAUNCH(false);
-      } else
       k_f_miller_s<kBlockFSM><<<(unsigned)((m + kBlockFSM - 1) / kBlockFSM), kBlockFSM, kSmemFMillerS, st>>>(d_in1, d_in2, mv, flag, gq, m, stride1, tab, rows);
     } else if (isf) k_f_miller<kBlockCCMiller><<<gm, kBlockCCMiller, 0, st>>>(d_in1, d_in2, mv, flag, m, stride1, tab, rows);
     else if (isg) k_g_miller<kBlockCCMiller><<<gm, kBlockCCMiller, 0, st>>>(d_in1, d_in2, mv, flag, m, stride1, tab, rows);
@@ -1526,8 +1470,6 @@ static double bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters
       if (mode == 0) k_fpmul_chain<kNA, true, 0><<<blocks, threads, 0, st>>>(out, in, iters);
       else if (mode == 2) k_fpmul_chain<kNA, true, 1><<<blocks, threads, 0, st>>>(out, in, iters);
       else if (mode == 3) k_fpmul_chain<kNA, true, 2><<<blocks, threads, 0, st>>>(out, in, iters);
-      else if (mode == 4) k_fpmul_slots<kNA, true, 128, 1><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
-      else if (mode == 5) k_fpmul_slots<kNA, true, 128, 2><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else if (mode == 6) k_fpmul_slots<kNA, true, 128, 3><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else if (mode == 7) k_fpmul_slots<kNA, true, 128, 4><<<blocks, threads, 2 * 64 * 128, st>>>(out, in, iters);
       else k_fpmul_slots<kNA, true, 128, 0><<<blocks, threads, smem, st>>>(out, in, iters);

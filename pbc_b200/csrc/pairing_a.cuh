@@ -12,7 +12,7 @@
 //   * the final exponentiation needs 1/N(f) and 1/(f0 f1) only (lucas_odd's P^2-4 equals
 //     -4 in1^2 on the norm-1 torus); both come from ONE inversion of N f0 f1, and that inversion
 //     is batched across pairings with Montgomery's trick (batch_invert kernel).
-// Pipeline per batch:  k_a_miller -> k_batch_invert -> k_a_finalexp.
+// Pipeline per batch:  k_a_miller9 -> k_batch_invert -> k_a_finalexp.
 #pragma once
 #include "slots.cuh"
 #include "a_steps.cuh"
@@ -26,13 +26,6 @@ struct AConsts {
   uint32_t two[16];     // Montgomery 2
 };
 __constant__ AConsts c_a;
-
-#ifndef PBC_A_FUSED
-#define PBC_A_FUSED 0
-#endif
-#ifndef PBC_A_W12
-#define PBC_A_W12 1     // Miller loop in weight-(1,2) coordinates (0: Jacobian)
-#endif
 
 constexpr int kNA = 16;        // 32-bit limbs of the 512-bit prime
 constexpr int kWA = 64;        // wire bytes per coordinate
@@ -59,191 +52,8 @@ __device__ __forceinline__ bool a_load_point(int sx, int sy, int st0, int st1, c
   return O::eq(st0, st1) && !O::is_zero(sy);
 }
 
-// The step in weight-(1,2) coordinates x = X/Z, y = Y/Z^2 (the doubling of Costello, Lange and
-// Naehrig for y^2 = x^3 + a x, re-derived for a = 1; tools/proto_a_w12.py checks it against the
-// reference fixtures):
-//   A = X^2, B = Y^2, C = Z^2;   X' = (A - C)^2,  Z' = 4 B,
-//   Y' = (2 (A + C)^2 - X') ((A - C + Y)^2 - B - X')
-//   line at phi(Q), up to a factor in F_q^*:  Re = X (A - C) + (3A + C) Z Qx,  Im = ((Y + Z)^2 - B - C) Qy
-// 10 multiplications + 7 squarings per step with the f update (Jacobian form above: 13 + 6), and no
-// Z^2 slot to maintain.
-template <class O>
-__device__ __forceinline__ void a_double_step_w12() {
-  // f = f^2
-  O::add(aT0, aF0, aF1);
-  O::sub(aT1, aF0, aF1);
-  O::mul(aF1, aF0, aF1);
-  O::dbl(aF1, aF1);
-  O::mul(aF0, aT0, aT1);
-  O::sqr(aT0, aX);                 // A
-  O::sqr(aT1, aY);                 // B
-  O::sqr(aT2, aZ);                 // C
-  O::sub(aT3, aT0, aT2);           // A - C
-  O::add(aT4, aT0, aT2);           // A + C
-  O::dbl(aT5, aT0);
-  O::add(aT5, aT5, aT4);           // 3A + C
-  O::mul(aT5, aT5, aZ);
-  O::mul(aT5, aT5, aQX);
-  O::mul(aT0, aX, aT3);
-  O::add(aT5, aT5, aT0);           // Re l
-  O::add(aT0, aY, aZ);
-  O::sqr(aT0, aT0);
-  O::sub(aT0, aT0, aT1);
-  O::sub(aT0, aT0, aT2);           // 2 Y Z
-  O::mul(aT0, aT0, aQY);           // Im l
-  O::dbl(aZ, aT1, 2);              // Z' = 4 B
-  O::sqr(aT4, aT4);                // (A + C)^2
-  O::sqr(aX, aT3);                 // X'
-  O::dbl(aT4, aT4);
-  O::sub(aT4, aT4, aX);            // E
-  O::add(aT2, aT3, aY);
-  O::sqr(aT2, aT2);
-  O::sub(aT2, aT2, aT1);
-  O::sub(aT2, aT2, aX);            // F = 2 Y (A - C)
-  O::mul(aY, aT4, aT2);            // Y'
-  a_fmul<O>(aF0, aF1, aT5, aT0, aT1, aT2, aT3);
-}
-
-// The same step with the additive operations folded into the multiply calls (Ops::fmul / fsqr):
-// 19 multiplier calls + 1 subtraction instead of 19 + 22 separate calls.  Values are identical.
-//   S1 = 2 F0 F1, S0 = (F0+F1)(F0-F1)                      f^2  (F0, F1 are free afterwards)
-//   M = Z2^2 + 3 X^2, Y2 = Y^2, S = 4 X Y2
-//   L0 = (M Z2) Qx + (X M - 2 Y2),  Z' = 2 Y Z,  L1 = (Z' Z2) Qy,  Z2' = Z'^2
-//   X' = M^2 - 2 S,  Y' = M (S - X') - 8 Y2^2
-//   f' = (S0 + i S1)(L0 + i L1)
-template <class O>
-__device__ __forceinline__ void a_double_step_fused() {
-  O::fmul(aT4, aF0, aF1, O::F_DBL(1), 0, 0, 0, 0);                        // S1
-  O::fmul(aT5, aF0, aF0, O::F_ADD_A | O::F_SUB_B, aF1, aF1, 0, 0);        // S0
-  O::fsqr(aT0, aX, 0, 0, 0);                                              // X^2
-  O::fsqr(aT0, aZ2, O::F_ADD_C1(3), aT0, 0);                              // M
-  O::fsqr(aT1, aY, 0, 0, 0);                                              // Y2
-  O::fmul(aT2, aX, aT1, O::F_DBL(2), 0, 0, 0, 0);                         // S
-  O::fmul(aT3, aT0, aZ2, 0, 0, 0, 0, 0);                                  // M Z2
-  O::fmul(aF0, aX, aT0, O::F_SUB_C1(2), 0, 0, aT1, 0);                    // X M - 2 Y2
-  O::fmul(aF0, aT3, aQX, O::F_ADD_C1(1), 0, 0, aF0, 0);                   // L0
-  O::fmul(aZ, aY, aZ, O::F_DBL(1), 0, 0, 0, 0);                           // Z'
-  O::fmul(aT3, aZ, aZ2, 0, 0, 0, 0, 0);
-  O::fmul(aF1, aT3, aQY, 0, 0, 0, 0, 0);                                  // L1
-  O::fsqr(aZ2, aZ, 0, 0, 0);
-  O::fsqr(aX, aT0, O::F_SUB_C1(2), aT2, 0);                               // X'
-  O::fsqr(aT1, aT1, O::F_DBL(3), 0, 0);                                   // 8 Y2^2
-  O::fmul(aY, aT0, aT2, O::F_SUB_B | O::F_SUB_C1(1), 0, aX, aT1, 0);      // Y'
-  O::fmul(aT0, aT5, aF0, 0, 0, 0, 0, 0);                                  // U0 = S0 L0
-  O::fmul(aT3, aT4, aF1, 0, 0, 0, 0, 0);                                  // U1 = S1 L1
-  O::fmul(aF1, aT5, aF0, O::F_ADD_A | O::F_ADD_B | O::F_SUB_C1(1) | O::F_SUB_C2(1), aT4, aF1, aT0, aT3);
-  O::sub(aF0, aT0, aT3);
-}
-
-// f: [2][4][n] uint4 (Montgomery F_q^2), dprod: [4][n] uint4 = N(f) f0 f1 (0 marks "output
-// identity"), save: [5][4][n] uint4 scratch for V1 and f1.
-template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK)
-k_a_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4* __restrict__ f,
-           uint4* __restrict__ dprod, uint4* __restrict__ save, size_t n) {
-  using O = Ops<kNA, true, BLOCK>;
-  size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
-  bool live = idx < n;
-  size_t src = live ? idx : 0;
-  bool okP = a_load_point<O>(aX, aY, aT0, aT1, P + src * (2 * kWA));
-  bool okQ = a_load_point<O>(aQX, aQY, aT0, aT1, Q + src * (2 * kWA));
-  bool valid = okP && okQ;
-
-  O::set_const(aZ, c_fp.one);
-  O::set_const(aZ2, c_fp.one);
-  O::set_const(aF0, c_fp.one);
-  uint32_t zero[kNA] = {0};
-  O::st(aF1, zero);
-
-  const int exp1 = c_a.exp1, exp2 = c_a.exp2;
-  for (int i = 0; i < exp2; i++) {
-    if (i == exp1 && live) {
-      // V1 = +-V, f1 = f or conj(f) ~ 1/f   (ecc/a_param.c:1162-1169)
-      if (c_a.sign1 < 0) { O::neg(aT0, aY); O::neg(aT1, aF1); }
-      else               { O::copy(aT0, aY); O::copy(aT1, aF1); }
-      O::st_global(save, 0, n, idx, aX);
-      O::st_global(save, 1, n, idx, aT0);
-      O::st_global(save, 2, n, idx, aZ);
-      O::st_global(save, 3, n, idx, aF0);
-      O::st_global(save, 4, n, idx, aT1);
-    }
-#if PBC_A_W12
-    a_double_step_w12<O>();
-#elif PBC_A_FUSED
-    a_double_step_fused<O>();
-#else
-    a_double_step<O>();
-#endif
-  }
-  if (!live) return;
-
-  // f *= f1
-  O::ld_global(aT3, save, 3, n, idx);
-  O::ld_global(aT4, save, 4, n, idx);
-  a_fmul<O>(aF0, aF1, aT3, aT4, aT0, aT1, aT2);
-#if PBC_A_W12
-  // chord through V = (X, Y, Z) and V1 = (X1, Y1, Z1) in weight-(1,2) coordinates, scaled by
-  // Z^2 Z1^2 (compute_abc_line :114-130):
-  //   a = Y Z1^2 - Y1 Z^2,  b = Z Z1 (X1 Z - X Z1),  c = X Z Y1 - Y X1 Z1
-  O::ld_global(aT0, save, 2, n, idx);          // Z1
-  O::ld_global(aT1, save, 0, n, idx);          // X1
-  O::ld_global(aT5, save, 1, n, idx);          // Y1
-  O::mul(aT2, aT1, aZ);                         // X1 Z
-  O::mul(aT3, aX, aT0);                         // X Z1
-  O::sub(aT2, aT2, aT3);
-  O::mul(aT2, aT2, aZ);
-  O::mul(aT4, aT2, aT0);                        // b
-  O::mul(aT3, aX, aZ);
-  O::mul(aT3, aT3, aT5);                        // X Z Y1
-  O::mul(aT1, aT1, aT0);                        // X1 Z1
-  O::mul(aT1, aT1, aY);                         // Y X1 Z1
-  O::sub(aT3, aT3, aT1);                        // c
-  O::sqr(aT0, aT0);                             // Z1^2
-  O::mul(aT0, aT0, aY);                         // Y Z1^2
-  O::sqr(aT1, aZ);                              // Z^2
-  O::mul(aT1, aT1, aT5);                        // Y1 Z^2
-  O::sub(aT2, aT0, aT1);                        // a
-  O::copy(aZ, aT3);                             // c where the common tail expects it
-#else
-  // chord through V=(X,Y,Z) and V1=(X1,Y1,Z1), scaled by Z^3 Z1^3 (compute_abc_line :114-130):
-  //   a = Y Z1^3 - Y1 Z^3,  b = X1 Z1 Z^3 - X Z Z1^3,  c = X Z Y1 - Y X1 Z1
-  O::ld_global(aT0, save, 2, n, idx);          // Z1
-  O::mul(aT1, aZ2, aZ);                         // Z^3
-  O::sqr(aT2, aT0);
-  O::mul(aT2, aT2, aT0);                        // Z1^3
-  O::mul(aT3, aX, aZ);                          // X Z
-  O::ld_global(aT4, save, 0, n, idx);          // X1
-  O::mul(aT4, aT4, aT0);                        // X1 Z1
-  O::ld_global(aT0, save, 1, n, idx);          // Y1
-  O::mul(aZ, aT3, aT0);                         // X Z Y1
-  O::mul(aZ2, aY, aT4);                         // Y X1 Z1
-  O::sub(aZ, aZ, aZ2);                          // c
-  O::mul(aT4, aT4, aT1);                        // X1 Z1 Z^3
-  O::mul(aT3, aT3, aT2);                        // X Z Z1^3
-  O::sub(aT4, aT4, aT3);                        // b
-  O::mul(aT2, aY, aT2);                         // Y Z1^3
-  O::mul(aT1, aT0, aT1);                        // Y1 Z^3
-  O::sub(aT2, aT2, aT1);                        // a
-#endif
-  O::mul(aT2, aT2, aQX);
-  O::sub(aT2, aZ, aT2);                         // Re l = c - a Qx
-  O::mul(aT4, aT4, aQY);                        // Im l = b Qy
-  a_fmul<O>(aF0, aF1, aT2, aT4, aT0, aT1, aT3);
-
-  // D = (f0^2 + f1^2) f0 f1;  invalid inputs publish D = 0 (-> identity)
-  O::sqr(aT0, aF0);
-  O::sqr(aT1, aF1);
-  O::add(aT0, aT0, aT1);
-  O::mul(aT1, aF0, aF1);
-  O::mul(aT0, aT0, aT1);
-  if (!valid) O::st(aT0, zero);
-  O::st_global(f, 0, n, idx, aF0);
-  O::st_global(f, 1, n, idx, aF1);
-  O::st_global(dprod, 0, n, idx, aT0);
-}
-
 // ---------------------------------------------------------------------------------------------
-// The same Miller loop on NINE slots (round 2).  k_a_miller above keeps 14 slots = 112 KB per
+// The Miller loop on NINE slots (round 2).  Round 1's kernel kept 14 slots = 112 KB per
 // 128-thread block: two blocks = 8 warps per SM, shared-memory bound (the top stall is the
 // fixed-latency wait of the carry chains).  Here
 //   * Q (used twice per step, as one operand of a multiplication) lives in a limb-major global array
@@ -262,10 +72,6 @@ k_a_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4* 
 //   f' = g (Re l + i Im l)
 // ---------------------------------------------------------------------------------------------
 enum A9Slot { nX, nY, nZ, nF0, nF1, nT0, nT1, nT2, nT3, kA9Slots };
-// PBC_A_LOCKSTEP = 1: block-wide barrier at the top of every Miller iteration (A/B experiment, see DESIGN.md)
-#ifndef PBC_A_LOCKSTEP
-#define PBC_A_LOCKSTEP 1
-#endif
 
 // qx, qy: this thread's Q coordinates in the global array (Montgomery form), vectors n apart.
 // a_step_9_line: on entry g = (nT0, nF1) and the f0 slot is free; on exit f' = g l in (nF0, nF1), V doubled.
@@ -378,20 +184,16 @@ __device__ __forceinline__ void a_chord_9(const uint4* save, const uint4* qx, co
   a_fmul_2t<O>(nF0, nF1, nT3, nT2, nT0, nT1);
 }
 
-// f, dprod, save as for k_a_miller; qm: [2][4][n] uint4 scratch (Montgomery-form Q)
+// f: [2][4][n] uint4 (Montgomery F_q^2), dprod: [4][n] uint4 = N(f) f0 f1 (0 marks "output
+// identity"), save: [5][4][n] uint4 scratch for V1 and f1, qm: [2][4][n] uint4 scratch (Montgomery-form Q)
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK)
 k_a_miller9(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4* __restrict__ f,
             uint4* __restrict__ dprod, uint4* __restrict__ save, uint4* __restrict__ qm, size_t n) {
   using O = Ops<kNA, true, BLOCK>;
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
-#if PBC_A_LOCKSTEP
   const bool live = idx < n;                 // every thread runs the loop: block-wide barrier inside
   if (!live) idx = 0;
-#else
-  if (idx >= n) return;                      // no block-wide barrier in this kernel
-  const bool live = true;
-#endif
   bool okP = a_load_point<O>(nX, nY, nT0, nT1, P + idx * (2 * kWA));
   bool okQ = a_load_point<O>(nT2, nT3, nT0, nT1, Q + idx * (2 * kWA));
   bool valid = okP && okQ;
@@ -409,9 +211,7 @@ k_a_miller9(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4*
 
   const int exp1 = c_a.exp1, exp2 = c_a.exp2;
   for (int i = 0; i < exp2; i++) {
-#if PBC_A_LOCKSTEP
     __syncthreads();                         // the loop is uniform: keep the block's warps in the same routine (instruction cache)
-#endif
     if (i == exp1 && live) {
       // V1 = +-V, f1 = f or conj(f) ~ 1/f   (ecc/a_param.c:1162-1169)
       if (c_a.sign1 < 0) { O::neg(nT0, nY); O::neg(nT1, nF1); }
@@ -445,142 +245,6 @@ k_a_miller9(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4*
 }
 
 // ---------------------------------------------------------------------------------------------
-// The same Miller loop on SEVEN slots.  g = f^2 and g0 + g1 go to a limb-major global array as soon as
-// they are computed, like Q, and the products f' = g l take them from there (Ops::mulg), so f needs no
-// slot during the line and doubling part.  The step of k_a_miller9, with the same products (11 M + 6 S),
-// on X, Y, Z and four temporaries; at most seven values are live (X, Y, Z, U, B, A', T).  f' and Y' end
-// in other slots than f and Y started in: the slot numbers are renamed every step instead of copied.
-// 7 x 64 B x 128 threads = 56 KB per block: FOUR blocks = 16 warps per SM (plus the 1 KB the runtime
-// reserves per block, exactly the 228 KB of an H100 SM).  Off by default (engine.cu, PBC_A_SLOTS): 2.5 %
-// fewer cycles than k_a_miller9, but a power-capped H100 lowers its clock by more (DESIGN.md 3.8).
-// ---------------------------------------------------------------------------------------------
-enum A7Slot { sX, sZ, sY0, sF00, sF10, sT00, sT10, kA7Slots };
-
-// one step.  On entry f = (f0, f1), V = (sX, y, sZ), t0 and t1 free; on exit the same for f', 2V.
-// g: this thread's column of the [3][4][ng] array that takes g0, g1 and g0 + g1.
-template <class O>
-__device__ __forceinline__ void a_double_step_7(int& y, int& f0, int& f1, int& t0, int& t1, uint4* g, size_t ng,
-                                                const uint4* qx, const uint4* qy, size_t n) {
-  const int a = f0, b = f1, c = t0, d = t1;
-  O::template mul2<true>(c, f0, f1, f0, f1);         // g0 = (f0 + f1)(f0 - f1)
-  O::mulx(d, f0, f1, O::MX_ADD_A, f0, 0, nullptr, 0);   // g1 = 2 f0 f1
-  O::add(a, c, d);
-  O::st_global(g, 0, ng, 0, c);
-  O::st_global(g, 1, ng, 0, d);
-  O::st_global(g, 2, ng, 0, a);                      // g0 + g1       (all four temporaries are free)
-  O::sqr(a, sX);                                     // A
-  O::sqr(b, y);                                      // B
-  O::sqr(c, sZ);                                     // C
-  O::sub(d, a, c);                                   // T = A - C
-  O::add(c, a, c);                                   // A' = A + C
-  O::dbl(a, c);
-  O::add(a, a, d);                                   // U = 3A + C
-  O::mulp(a, a, sZ);
-  O::mulg(a, a, qx, n);                              // U Z Qx
-  O::mulp(sX, sX, d);                                // X T
-  O::add(a, a, sX);                                  // Re l                   (X slot is free)
-  O::sqr(sX, d);                                     // X' = T^2
-  O::sqr(c, c);
-  O::dbl(c, c);
-  O::sub(c, c, sX);                                  // E = 2 A'^2 - X'
-  O::add(d, d, y);
-  O::sqr(d, d);
-  O::sub(d, d, b);
-  O::sub(d, d, sX);                                  // F = (T + Y)^2 - B - X'
-  O::mulp(c, c, d);                                  // Y'
-  O::mulp(d, y, sZ);
-  O::dbl(d, d);
-  O::mulg(d, d, qy, n);                              // Im l = 2 Y Z Qy
-  O::dbl(sZ, b, 2);                                  // Z' = 4 B
-  O::mulx(b, a, 0, O::MX_ADD_A | O::MX_GLOBAL_B, d, 0, g + 8 * ng, ng);   // (Re l + Im l)(g0 + g1)
-  O::mulg(a, a, g, ng);                              // g0 Re l
-  O::mulg(d, d, g + 4 * ng, ng);                     // g1 Im l
-  O::sub(y, a, d);                                   // f0'
-  O::sub(b, b, a);
-  O::sub(b, b, d);                                   // f1'
-  f0 = y; y = c; f1 = b; t0 = a; t1 = d;
-}
-
-// f, dprod, save, qm as for k_a_miller9; g: [3][4][ng] uint4 scratch, ng = n rounded up to BLOCK: every
-// thread, the padding threads of the last block included, owns a column
-template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, 4)
-k_a_miller7(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4* __restrict__ f,
-            uint4* __restrict__ dprod, uint4* __restrict__ save, uint4* __restrict__ qm, uint4* __restrict__ g,
-            size_t n) {
-  using O = Ops<kNA, true, BLOCK>;
-  size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
-  const size_t ng = (size_t)gridDim.x * BLOCK;
-  uint4* gcol = g + idx;
-#if PBC_A_LOCKSTEP
-  const bool live = idx < n;                 // every thread runs the loop: block-wide barrier inside
-  if (!live) idx = 0;
-#else
-  if (idx >= n) return;
-  const bool live = true;
-#endif
-  int y = sY0, f0 = sF00, f1 = sF10, t0 = sT00, t1 = sT10;
-  bool okP = a_load_point<O>(sX, y, t0, t1, P + idx * (2 * kWA));
-  bool okQ = a_load_point<O>(f0, f1, t0, t1, Q + idx * (2 * kWA));
-  bool valid = okP && okQ;
-  if (live) {
-    O::st_global(qm, 0, n, idx, f0);
-    O::st_global(qm, 1, n, idx, f1);
-  }
-  const uint4* qx = qm + idx;
-  const uint4* qy = qm + 4 * n + idx;
-
-  O::set_const(sZ, c_fp.one);
-  O::set_const(f0, c_fp.one);
-  uint32_t zero[kNA] = {0};
-  O::st(f1, zero);
-
-  const int exp1 = c_a.exp1, exp2 = c_a.exp2;
-  for (int i = 0; i < exp2; i++) {
-#if PBC_A_LOCKSTEP
-    __syncthreads();
-#endif
-    if (i == exp1 && live) {
-      // V1 = +-V, f1 = f or conj(f) ~ 1/f   (ecc/a_param.c:1162-1169)
-      if (c_a.sign1 < 0) { O::neg(t0, y); O::neg(t1, f1); }
-      else               { O::copy(t0, y); O::copy(t1, f1); }
-      O::st_global(save, 0, n, idx, sX);
-      O::st_global(save, 1, n, idx, t0);
-      O::st_global(save, 2, n, idx, sZ);
-      O::st_global(save, 3, n, idx, f0);
-      O::st_global(save, 4, n, idx, t1);
-    }
-    a_double_step_7<O>(y, f0, f1, t0, t1, gcol, ng, qx, qy, n);
-  }
-  if (!live) return;
-
-  // f *= chord, then f *= f1 (the order of the two factors does not change the product).  f is parked in
-  // the output array while the chord takes four temporaries.
-  O::st_global(f, 0, n, idx, f0);
-  O::st_global(f, 1, n, idx, f1);
-  a_chord_line<O>(sX, y, sZ, f0, f1, t0, t1, save, qx, qy, n, idx);    // Re l in t1, Im l in t0
-  O::ld_global(sX, f, 0, n, idx);
-  O::ld_global(y, f, 1, n, idx);
-  a_fmul_2t<O>(sX, y, t1, t0, f0, f1);
-  O::ld_global(t0, save, 3, n, idx);
-  O::ld_global(t1, save, 4, n, idx);
-  a_fmul_2t<O>(sX, y, t0, t1, f0, f1);
-  f0 = sX;
-  f1 = y;
-
-  // D = (f0^2 + f1^2) f0 f1;  invalid inputs publish D = 0 (-> identity)
-  O::sqr(t0, f0);
-  O::sqr(t1, f1);
-  O::add(t0, t0, t1);
-  O::mulp(t1, f0, f1);
-  O::mulp(t0, t0, t1);
-  if (!valid) O::st(t0, zero);
-  O::st_global(f, 0, n, idx, f0);
-  O::st_global(f, 1, n, idx, f1);
-  O::st_global(dprod, 0, n, idx, t0);
-}
-
-// ---------------------------------------------------------------------------------------------
 // Shared Miller accumulator (a_pairings_affine, ecc/a_param.c:1283-1383: ONE f for the n pairs of a
 // product, f <- f^2 once per step, then f <- f l_j for every pair).  One thread owns M consecutive pairs
 // of one product: per step it squares f once and runs the line / doubling part of the nine-slot step
@@ -597,13 +261,8 @@ k_a_miller9_shared(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q,
                    uint4* __restrict__ vj, size_t n_thr, size_t M) {
   using O = Ops<kNA, true, BLOCK>;
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
-#if PBC_A_LOCKSTEP
   const bool live = idx < n_thr;
   if (!live) idx = 0;
-#else
-  if (idx >= n_thr) return;
-  const bool live = true;
-#endif
   const size_t np = n_thr * M, p0 = idx * M;
   bool valid = true;
   for (size_t j = 0; j < M; j++) {
@@ -626,9 +285,7 @@ k_a_miller9_shared(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q,
 
   const int exp1 = c_a.exp1, exp2 = c_a.exp2;
   for (int i = 0; i < exp2; i++) {
-#if PBC_A_LOCKSTEP
     __syncthreads();
-#endif
     if (i == exp1 && live) {
       // f1 = f or conj(f) ~ 1/f, once per thread (kept with the thread's first pair)
       if (c_a.sign1 < 0) O::neg(nT1, nF1); else O::copy(nT1, nF1);
@@ -683,7 +340,7 @@ k_a_miller9_shared(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q,
 // ---------------------------------------------------------------------------------------------
 // element_prod_pairing (include/pbc_pairing.h:153-171 -> a_pairings_affine, ecc/a_param.c:1283-1383).
 // The reference shares one accumulator f between the k Miller loops; here every (P_j, Q_j) pair
-// runs its own k_a_miller thread (k times more parallelism for a 2^16-output batch) and the k
+// runs its own k_a_miller9 thread (k times more parallelism for a 2^16-output batch) and the k
 // Miller values of one output are multiplied afterwards.  prod_j f_j differs from the reference's
 // shared accumulator only by factors in F_q^*, which the final exponentiation kills.
 //   f_in [2][4][n_in], d_in [4][n_in]  (n_in = n_out * k; d = 0 marks an O / off-curve input),

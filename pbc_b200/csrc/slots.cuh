@@ -67,7 +67,7 @@ struct Ops {
     fp_sqr<N, FULL>(x, x);
     st(d, x);
   }
-  // ---- ONE multiplier routine for the kernels that need operand variants (k_a_miller9, k_a_miller7) ----
+  // ---- ONE multiplier routine for the kernels that need operand variants (k_a_miller9, k_a_miller9_shared) ----
   // d = x * y with  x = a [+ a2],  y = b [+ b2 | - b2]  or  y = the element at g (limb-major global
   // array, vectors n apart: a value used once or twice per loop iteration lives in L2 instead of a
   // slot).  All branches are warp-uniform.  One copy of the 528-product body instead of one per
@@ -191,57 +191,6 @@ struct Ops {
 #pragma unroll
     for (int k = 0; k < N; k++) y[k] = c[k];
     fp_sub<N>(x, x, y);
-    st(d, x);
-  }
-  // ---- fused multiply: d = ((a [+- a2]) * (b [+- b2]) [+- n1 c1] [+- n2 c2]) * 2^k ----
-  // One call replaces a multiplication and the additive operations around it (each of which
-  // would otherwise be its own call with its own shared-memory round trip).  `f` is built with
-  // the F_* helpers below; all branches on it are warp-uniform.
-  static constexpr uint32_t F_ADD_A = 1u, F_SUB_A = 2u, F_ADD_B = 4u, F_SUB_B = 8u;
-  static __host__ __device__ constexpr uint32_t F_ADD_C1(uint32_t n) { return n << 4; }
-  static __host__ __device__ constexpr uint32_t F_SUB_C1(uint32_t n) { return (n << 4) | 0x80u; }
-  static __host__ __device__ constexpr uint32_t F_ADD_C2(uint32_t n) { return n << 8; }
-  static __host__ __device__ constexpr uint32_t F_SUB_C2(uint32_t n) { return (n << 8) | 0x800u; }
-  static __host__ __device__ constexpr uint32_t F_DBL(uint32_t k) { return k << 12; }
-
-  static __device__ __forceinline__ void post_ops(uint32_t* x, uint32_t f, int c1, int c2) {
-    uint32_t y[N];
-    if (f & 0x70u) {
-      ld(y, c1);
-      for (uint32_t i = (f >> 4) & 7u; i; i--) {
-        if (f & 0x80u) fp_sub<N>(x, x, y); else fp_add<N, FULL>(x, x, y);
-      }
-    }
-    if (f & 0x700u) {
-      ld(y, c2);
-      for (uint32_t i = (f >> 8) & 7u; i; i--) {
-        if (f & 0x800u) fp_sub<N>(x, x, y); else fp_add<N, FULL>(x, x, y);
-      }
-    }
-    for (uint32_t i = (f >> 12) & 3u; i; i--) fp_add<N, FULL>(x, x, x);
-  }
-  static __device__ __noinline__ void fmul(int d, int a, int b, uint32_t f, int a2, int b2, int c1, int c2) {
-    uint32_t x[N], y[N];
-    ld(y, b);
-    if (f & (F_ADD_B | F_SUB_B)) {
-      ld(x, b2);
-      if (f & F_ADD_B) fp_add<N, FULL>(y, y, x); else fp_sub<N>(y, y, x);
-    }
-    ld(x, a);
-    if (f & (F_ADD_A | F_SUB_A)) {
-      uint32_t z[N];
-      ld(z, a2);
-      if (f & F_ADD_A) fp_add<N, FULL>(x, x, z); else fp_sub<N>(x, x, z);
-    }
-    fp_mul<N, FULL>(x, x, y);
-    post_ops(x, f, c1, c2);
-    st(d, x);
-  }
-  static __device__ __noinline__ void fsqr(int d, int a, uint32_t f, int c1, int c2) {
-    uint32_t x[N];
-    ld(x, a);
-    fp_sqr<N, FULL>(x, x);
-    post_ops(x, f, c1, c2);
     st(d, x);
   }
   static __device__ __noinline__ void add(int d, int a, int b) {

@@ -11,9 +11,6 @@
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
-#include <condition_variable>
-#include <mutex>
-#include <thread>
 
 struct uint2 { uint32_t x, y; };
 struct alignas(16) uint4 { uint32_t x, y, z, w; };
@@ -32,66 +29,21 @@ inline int& current_device() { static thread_local int d = 0; return d; }
 inline int device_count() { const char* e = getenv("PBC_SIM_DEVICES"); int n = e ? atoi(e) : 1; return n > 0 ? n : 1; }
 inline uint64_t& launches() { static uint64_t n = 0; return n; }
 // optional cap on simulated threads per launch (0 = all): kernels whose padding threads keep
-// computing (k_a_miller's `live` pattern) would otherwise cost a full block per launch
+// computing (k_a_miller9's `live` pattern) would otherwise cost a full block per launch
 inline size_t& live_threads() { static size_t n = 0; return n; }
 // shared memory is poisoned at the start of every block and device allocations at birth, so a
 // kernel that reads what it never wrote sees garbage here as it would on the GPU
 inline void (*&poison_shared())() { static void (*f)() = nullptr; return f; }
-// this host thread's own shared-memory buffer (set by the generated source, which owns the buffer)
-inline void* (*&shared_self_fn())() { static void* (*f)() = nullptr; return f; }
-inline void* shared_self() { return shared_self_fn() ? shared_self_fn()() : nullptr; }
-// ---- lane pairs ----
-// A kernel whose adjacent lanes (2j, 2j+1) cooperate through shared memory, __syncwarp() and
-// __shfl_xor_sync(.., 1) (the pair kernels of pairing_f_pair.cuh) is launched with pair_mode() set: the two
-// lanes of a pair then run on two host threads that meet at every __syncwarp / shuffle; pairs still run one
-// after the other.  Both lanes must reach the same sequence of barriers (true of those kernels: one
-// instruction stream, the lane parity only selects operands).
-struct PairCtx {
-  std::mutex m;
-  std::condition_variable cv;
-  int waiting = 0;
-  unsigned long long phase = 0;
-  uint32_t box[2] = {0, 0};
-  void sync() {
-    std::unique_lock<std::mutex> lk(m);
-    unsigned long long ph = phase;
-    if (++waiting == 2) { waiting = 0; phase++; cv.notify_all(); }
-    else cv.wait(lk, [&] { return phase != ph; });
-  }
-};
-inline bool& pair_mode() { static thread_local bool v = false; return v; }
-inline PairCtx*& pair_ctx() { static thread_local PairCtx* p = nullptr; return p; }
-// the shared-memory buffer a simulated thread sees: its host thread's own, or (second lane of a pair) the first lane's
-inline void*& shared_override() { static thread_local void* p = nullptr; return p; }
-
 template <class F>
 inline void launch(dim3 grid, dim3 block, F&& body) {
   launches()++;
   gdim() = grid; bdim() = block;
   size_t done = 0;
-  const bool pairs = pair_mode();
   for (unsigned b = 0; b < grid.x; b++) {
     if (poison_shared()) poison_shared()();
     for (unsigned t = 0; t < block.x; t++) {
       if (live_threads() && done >= live_threads()) return;
       bid() = dim3(b); tid() = dim3(t);
-      if (pairs && t + 1 < block.x) {
-        PairCtx ctx;
-        void* shared = shared_self();
-        const dim3 g = grid, bd = block;
-        std::thread other([&, b, t, g, bd, shared] {
-          gdim() = g; bdim() = bd; bid() = dim3(b); tid() = dim3(t + 1);
-          pair_ctx() = &ctx; shared_override() = shared;
-          body();
-          pair_ctx() = nullptr; shared_override() = nullptr;
-        });
-        pair_ctx() = &ctx;
-        body();
-        other.join();
-        pair_ctx() = nullptr;
-        t++; done += 2;
-        continue;
-      }
       body();
       done++;
     }
@@ -104,18 +56,7 @@ inline void launch(dim3 grid, dim3 block, F&& body) {
 #define gridDim (::cusim::gdim())
 
 static inline void __syncthreads() {}
-static inline void __syncwarp() { if (::cusim::pair_ctx()) ::cusim::pair_ctx()->sync(); }
-// only the lane-pair exchange (mask 1) is simulated
-static inline uint32_t __shfl_xor_sync(unsigned, uint32_t v, int lane_mask) {
-  ::cusim::PairCtx* c = ::cusim::pair_ctx();
-  if (!c || lane_mask != 1) abort();
-  const unsigned me = threadIdx.x & 1u;
-  c->box[me] = v;
-  c->sync();
-  uint32_t r = c->box[me ^ 1u];
-  c->sync();
-  return r;
-}
+static inline void __syncwarp() {}
 static inline uint32_t __funnelshift_r(uint32_t lo, uint32_t hi, uint32_t s) {
   return (uint32_t)((((uint64_t)hi << 32) | lo) >> (s & 31));
 }

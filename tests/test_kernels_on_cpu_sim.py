@@ -59,7 +59,8 @@ def test_gpu_parity_tests_pass_on_the_simulator(sim):
     cases sized for a GPU (2^14 .. 2^18 outputs), the device-pointer entry points (they take
     torch.cuda tensors) and the C programs of the shim (they link the real library)"""
     files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_towers.py", "test_gpu_type_a.py", "test_gpu_type_a1.py",
-                                                       "test_gpu_type_fd.py", "test_gpu_group_ops.py", "test_gpu_zz_a1_group_ops.py")]
+                                                       "test_gpu_type_fd.py", "test_gpu_edge_cases.py", "test_gpu_group_ops.py",
+                                                       "test_gpu_zz_a1_group_ops.py")]
     cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
            "-k", "not large_batch and not device_pointer and not tiles and not across_blocks"] + files
     try:
@@ -87,27 +88,6 @@ def test_kernel_variants_give_the_same_bytes(tmp_path):
                 "-DPBC_FQ_ACC=0", "-DPBC_FS_CYC_ONE=0", "-DPBC_FQ_CALL_OS=0", "-DPBC_MULW_MAD=0", "-DPBC_FS_ONE_QMUL=1")
     res = _battery(so)
     assert len(res) >= 38 and all(res.values()), {k: v for k, v in res.items() if not v}
-
-
-def test_type_f_lane_pair_kernels_give_the_same_bytes(tmp_path):
-    """PBC_F_PAIR = 1 (pairing_f_pair.cuh: k_f_prep + k_f_miller_p, two lanes per pairing meeting at __syncwarp; no faster
-    than the slot kernel and kept off, engine.cu says why): the type F / D fixtures and the edge cases through that build.  The simulator
-    runs the two lanes of a pair on two host threads (tests/host/cuda_sim.hpp), so a missing barrier shows up here."""
-    if not shutil.which("g++"):
-        pytest.skip("no g++")
-    so = _build(tmp_path, "-DPBC_F_PAIR=1", "-DPBC_FP_SWIZZLE=1")     # with the bank swizzle of the slots (measured, off by default)
-    files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_type_fd.py", "test_gpu_edge_cases.py")]
-    cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
-           "-k", "not large_batch and not device_pointer and not tiles and not across_blocks"] + files
-    try:
-        import xdist  # noqa: F401
-        cmd += ["-n", str(max(1, min(8, len(os.sched_getaffinity(0)))))]
-    except Exception:
-        pass
-    out = subprocess.run(cmd, env=_env(so), capture_output=True, text=True, timeout=1500, cwd=ROOT)
-    tail = out.stdout.strip().splitlines()[-1] if out.stdout.strip() else out.stderr[-500:]
-    assert out.returncode == 0, out.stdout[-3000:]
-    assert int(tail.split(" passed")[0].split()[-1]) >= 150, tail
 
 
 def test_multiplier_work_counted_by_the_simulator_matches_bench(sim):

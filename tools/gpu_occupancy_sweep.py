@@ -2,7 +2,8 @@
 
 k_fpmul_slots (the 512-bit multiplier the type A kernels call, through shared-memory slots) launched
 with its dynamic shared memory padded to the footprint of a pairing kernel: 72 KB is the nine-slot
-Miller kernel, 56 KB the seven-slot one, 32 KB and 16 KB leave registers as the limit.  The blocks per
+Miller kernel, 56 KB the footprint of a seven-slot one (four blocks per SM), 32 KB and 16 KB leave
+registers as the limit.  The blocks per
 SM of each size come from the device (cudaOccupancyMaxActiveBlocksPerMultiprocessor).  Prints one JSON
 object per line; the first names the GPU and its power limit."""
 import json

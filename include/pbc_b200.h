@@ -8,6 +8,15 @@
  *   type A  (param/a.param)     G1 128 B   G2 128 B   GT 128 B     x || y, 64-byte big-endian F_q
  *   type F  (param/f.param)     G1  40 B   G2  80 B   GT 240 B     20-byte big-endian F_q
  *   type D  (param/d159.param)  G1  40 B   G2 120 B   GT 120 B     20-byte big-endian F_q
+ *   type D, 160..255-bit q      G1 2wb     G2 6wb     GT 6wb       wb = ceil(bits(q)/8) = 22..32-byte F_q;
+ *                                                                  Zr ceil(bits(r)/8), r below 2^255:
+ *     d277699-175-167.param     G1  44 B   G2 132 B   GT 132 B     Zr 21 B
+ *     d278027-190-181.param     G1  48 B   G2 144 B   GT 144 B     Zr 23 B
+ *     d105171-196-185.param     G1  50 B   G2 150 B   GT 150 B     Zr 24 B
+ *     d201.param                G1  52 B   G2 156 B   GT 156 B     Zr 23 B
+ *     d224.param                G1  56 B   G2 168 B   GT 168 B     Zr 28 B
+ *     (type D q of 153..159 bits runs five-limb kernels, 160..255 bits eight-limb ones; other q are
+ *     rejected at init)
  *   type G  (param/g149.param)  G1  38 B   G2 190 B   GT 190 B     19-byte big-endian F_q
  *   type A1 (param/a1.param)    G1 260 B   G2 260 B   GT 260 B     ceil(bits(p)/8) = 130-byte F_p; any
  *                                                                  p = l n - 1 below 2^1087 is accepted
@@ -158,7 +167,8 @@ int pbc_b200_is_almost_coddh(pbc_b200_pairing_t *p, unsigned char *flags, const 
  * ecc/curve.c:455-482 with pbc_mpz_from_hash, arith/field.c:643-668): out[i] = the G1 element the
  * reference derives from the `len` bytes at data + i*len -- x from the hash, x <- x^2 + 1 until
  * x^3 + ax + b is a square, the odd square root, times the cofactor of G1.  Needs q = 3 mod 4 or
- * q = 5 mod 8 (a.param, f.param, d159.param all qualify). */
+ * q = 5 mod 8 (a.param, f.param, d159.param all qualify); type D with 160..255-bit q takes any q
+ * (Tonelli-Shanks where q = 1 mod 8: the four bundled sets other than d201). */
 int pbc_b200_g1_from_hash(pbc_b200_pairing_t *p, unsigned char *out, const unsigned char *data,
                           size_t len, size_t n);
 int pbc_b200_g1_from_hash_device(pbc_b200_pairing_t *p, void *d_out, const void *d_data, size_t len,

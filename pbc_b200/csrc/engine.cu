@@ -31,6 +31,26 @@
 #include "group_a.cuh"
 #include "group_a1.cuh"
 #include "group_cc.cuh"
+#include "engine_d_wide.h"
+
+#if defined(PBC_HOST_SIM) && !defined(PBC_HOST_SIM_D_WIDE)
+// A CPU simulator made from this translation unit alone has no eight-limb type D instance (that is
+// engine_d_wide.cu, a second one): type D with 160..255-bit q initialises, but its first device call
+// fails with an error instead of reaching a kernel.  tests/host/make_host_sim_d_wide.py appends the
+// instance and defines PBC_HOST_SIM_D_WIDE.
+namespace pbcb200_dw {
+int dw_upload(const DWideConsts&) { return -2; }
+void dw_miller(const uint8_t*, const uint8_t*, uint32_t*, uint32_t*, size_t, size_t, const uint32_t*, size_t, cudaStream_t) {}
+void dw_prod(const uint32_t*, const uint32_t*, uint32_t*, uint32_t*, size_t, size_t, size_t, cudaStream_t) {}
+void dw_finalexp(const uint32_t*, const uint32_t*, uint8_t*, size_t, cudaStream_t) {}
+void dw_pp_init(const uint8_t*, uint32_t*, size_t, cudaStream_t) {}
+void dw_group(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
+void dw_from_hash(const uint8_t*, int, uint8_t*, size_t, cudaStream_t) {}
+void dw_decompress(const uint8_t*, uint8_t*, size_t, cudaStream_t) {}
+void dw_tower_op(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
+void dw_fq_op(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
+}  // namespace pbcb200_dw
+#endif
 
 namespace pbcb200 {
 __global__ void k_fqmul_chain(uint32_t* __restrict__ out, const uint32_t* __restrict__ in, int iters, int mode);
@@ -140,6 +160,16 @@ struct pbc_b200_pairing_s {
 #endif
   FConsts f;
   DConsts d;
+  // type d with 160..255-bit q: the eight-limb instance (engine_d_wide.cu) and its constants; fp and
+  // hash above serve both instances (their layout does not depend on the limb count)
+  bool dwide = false;
+  CCConstsT<pbcb200_dw::kLimbs> dw_cc;
+  DConstsT<pbcb200_dw::kLimbs> dw_d;
+  ZrConstsT<pbcb200_dw::kLimbs> dw_zr;
+  FqWideConstsT<pbcb200_dw::kLimbs> dw_x;
+#if PBC_CC_NAF
+  CCNaf dw_naf;
+#endif
   GConsts g;
   ZrConsts zr;
   HashConsts hash;
@@ -208,7 +238,7 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
     return n_out * (2 + 1 + 1) * fq + (size_t)(3 * (p->a.exp2 + 1) * kNA + 4) * 4;
   }
   // types f, d: Miller values [W][n] words + one flag word each; products add the reduced arrays
-  size_t W = p->type == 'f' ? kF12Words : (p->type == 'g' ? kF10Words : kF6DWords);
+  size_t W = p->type == 'f' ? kF12Words : (p->type == 'g' ? kF10Words : 6 * (size_t)p->nlimbs);
   size_t n_in = job.mode == kProd ? n_out * job.k : n_out;
   size_t bytes = n_in * (W + 1) * 4;
   if (p->type == 'f') bytes += n_in * (size_t)kFGWords * 4;   // Q, P of the slot-machine Miller kernel
@@ -221,7 +251,8 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
 // strictly between the top digit and digit 0 (miller_cc_walk)
 static size_t cc_table_rows_compute(const pbc_b200_pairing_s* p) {
   BigUInt r;
-  for (int i = kNS; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->cc.r[i]);
+  if (p->dwide) for (int i = pbcb200_dw::kLimbs; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->dw_cc.r[i]);
+  else for (int i = kNS; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->cc.r[i]);
 #if PBC_CC_NAF
   std::vector<int8_t> dg = naf_digits(r);
   size_t rows = dg.size() - 1;
@@ -233,7 +264,7 @@ static size_t cc_table_rows_compute(const pbc_b200_pairing_s* p) {
   return rows;
 }
 static size_t cc_table_rows(const pbc_b200_pairing_s* p) { return p->cc_rows; }
-static size_t cc_table_bytes(const pbc_b200_pairing_s* p) { return (cc_table_rows(p) * 3 * kNS + 4) * 4; }
+static size_t cc_table_bytes(const pbc_b200_pairing_s* p) { return (cc_table_rows(p) * 3 * (size_t)p->nlimbs + 4) * 4; }
 
 static size_t in1_elems(const Job& job, size_t n_out) {
   return job.mode == kProd ? n_out * job.k : (job.mode == kPP ? 1 : n_out);
@@ -394,11 +425,12 @@ static void fill_hash(pbc_b200_pairing_s* p, const BigUInt& q, const BigUInt& co
 static void to_mont(uint32_t* out, const BigUInt& x, const BigUInt& q, int n) {
   ((x % q).shl(32 * (size_t)n) % q).to_words(out, n);
 }
-static void fill_cc(CCConsts* c, const BigUInt& A, const BigUInt& B, const BigUInt& r, const BigUInt& q) {
+template <int NS>
+static void fill_cc(CCConstsT<NS>* c, const BigUInt& A, const BigUInt& B, const BigUInt& r, const BigUInt& q) {
   memset(c, 0, sizeof *c);
-  to_mont(c->A, A, q, kNS);
-  to_mont(c->B, B, q, kNS);
-  r.to_words(c->r, kNS);
+  to_mont(c->A, A, q, NS);
+  to_mont(c->B, B, q, NS);
+  r.to_words(c->r, NS);
   c->rbits = (uint32_t)r.bits();
   c->a_is_zero = (A % q).is_zero() ? 1u : 0u;
 }
@@ -598,44 +630,32 @@ static int init_type_f(pbc_b200_pairing_s* p, const std::map<std::string, std::s
   return 0;
 }
 
-// d_init_pairing (ecc/d_param.c:993-1095), k = 6
-static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::string>& tab) {
-  BigUInt q, r, a, b, nqr, c0, c1, c2;
-  int k = 0;
-  if (!get_big(tab, "q", &q) || !get_big(tab, "r", &r) || !get_big(tab, "a", &a) || !get_big(tab, "b", &b) ||
-      !get_int(tab, "k", &k) || !get_big(tab, "nqr", &nqr) || !get_big(tab, "coeff0", &c0) ||
-      !get_big(tab, "coeff1", &c1) || !get_big(tab, "coeff2", &c2)) return 1;
-  if (k != 6) return fail("type d: only embedding degree 6 is on the GPU hot path (got k = %d)", k);
-  if (q.bits() > 159 || q.bits() < 153) return fail("type d: this build supports 153..159-bit q (20-byte coordinates; got %zu bits)", q.bits());
-  if (r.bits() > 160 || r.bits() < 3) return fail("type d: bad group order");
-  p->type = 'd';
-  memset(&p->zr, 0, sizeof p->zr);
-  r.to_words(p->zr.r, 5);
-  p->zr.zlen = (uint32_t)((r.bits() + 7) / 8);
-  p->zr_len = (int)p->zr.zlen;
-  p->nlimbs = kNS;
-  p->full = false;
-  p->g1_len = 2 * kWS; p->g2_len = 6 * kWS; p->gt_len = 6 * kWS;
-  fill_fp_consts(&p->fp, q, kNS);
-  fill_cc(&p->cc, a, b, r, q);
-  {
-    BigUInt hco(1);
-    auto ith = tab.find("h");
-    if (ith != tab.end()) BigUInt::from_dec(ith->second, &hco);
-    fill_hash(p, q, hco);                  // G1 cofactor = h (ecc/d_param.c:1016)
-  }
-  DConsts& c = p->d;
+// d_init_pairing (ecc/d_param.c:993-1095), k = 6.
+// Two instances of the type D kernels.  153..159-bit q (20-byte coordinates): five limbs, engine.cu's own
+// kernels.  160..255-bit q (22..32-byte coordinates): eight limbs, R = 2^256 (engine_d_wide.cu).  The
+// upper end is where the eight-limb code stops being exact, the least of:
+//   * mont_mul<8, false>, fp_add<8, false>, fp_halve (FULL = false, no carry word): a + q <= 2^256 for the
+//     operands they see, all canonical (< q): q < 2^255;
+//   * the lazy F_q^3 product (pairing_d.cuh, PBC_D_LAZY, internal basis): fq_add_nr sums below 2q < 2^256
+//     fit the limbs, every value handed to the reduction lies in (0, 4 q^2), and redc_wide takes t < 2 q R:
+//     4 q^2 < 2 q 2^256, again q < 2^255;
+//   * fq_from_wire: any 32-byte input is below R and mont_mul_ps(x, R^2 mod q) of it is below 2q: q < 2^255;
+//   * the signed-digit table of r (CCNaf, 256 digits) and the eight-word scalars: r < 2^255.
+// So q < 2^255 (at most 255 bits) and r of at most 255 bits; the largest bundled set, d224, has 224.
+template <int NS>
+static int fill_type_d(pbc_b200_pairing_s* p, DConstsT<NS>& c, const BigUInt& q, const BigUInt& r, const BigUInt& a,
+                       const BigUInt& b, const BigUInt& nqr, const BigUInt& c0, const BigUInt& c1, const BigUInt& c2) {
   memset(&c, 0, sizeof c);
   BigUInt v = nqr % q, vinv = BigUInt::invmod(v, q), one(1);
   BigUInt v2 = BigUInt::mulmod(v, v, q);
-  to_mont(c.nqr, v, q, kNS);
-  to_mont(c.nqrinv, vinv, q, kNS);
-  to_mont(c.nqrinv2, BigUInt::mulmod(vinv, vinv, q), q, kNS);
-  to_mont(c.twist_a, BigUInt::mulmod(a % q, v2, q), q, kNS);
-  to_mont(c.twist_b, BigUInt::mulmod(b % q, BigUInt::mulmod(v2, v, q), q), q, kNS);
-  to_mont(c.two, BigUInt(2), q, kNS);
-  (q * q).to_words(c.qsqm[0], 2 * kNS);
-  (q * q * BigUInt(2)).to_words(c.qsqm[1], 2 * kNS);
+  to_mont(c.nqr, v, q, NS);
+  to_mont(c.nqrinv, vinv, q, NS);
+  to_mont(c.nqrinv2, BigUInt::mulmod(vinv, vinv, q), q, NS);
+  to_mont(c.twist_a, BigUInt::mulmod(a % q, v2, q), q, NS);
+  to_mont(c.twist_b, BigUInt::mulmod(b % q, BigUInt::mulmod(v2, v, q), q), q, NS);
+  to_mont(c.two, BigUInt(2), q, NS);
+  (q * q).to_words(c.qsqm[0], 2 * NS);
+  (q * q * BigUInt(2)).to_words(c.qsqm[1], 2 * NS);
   HostF3Field Kref{q, {c0 % q, c1 % q, c2 % q}};
   HostF3 x;
   x.c[1] = one;
@@ -657,24 +677,24 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
       BigUInt lami = BigUInt::invmod(lam, q);
       BigUInt pc = BigUInt::mulmod(P, BigUInt::mulmod(lami, lami, q), q);
       c.nice = 1;
-      to_mont(c.pcoef, pc, q, kNS);
-      to_mont(c.bs, s0, q, kNS);
-      to_mont(c.bs2, BigUInt::mulmod(s0, s0, q), q, kNS);
-      to_mont(c.b2s, BigUInt::addmod(s0, s0, q), q, kNS);
-      to_mont(c.blam, lam, q, kNS);
-      to_mont(c.blam2, lam2, q, kNS);
-      to_mont(c.blami, lami, q, kNS);
-      to_mont(c.blami2, BigUInt::mulmod(lami, lami, q), q, kNS);
+      to_mont(c.pcoef, pc, q, NS);
+      to_mont(c.bs, s0, q, NS);
+      to_mont(c.bs2, BigUInt::mulmod(s0, s0, q), q, NS);
+      to_mont(c.b2s, BigUInt::addmod(s0, s0, q), q, NS);
+      to_mont(c.blam, lam, q, NS);
+      to_mont(c.blam2, lam2, q, NS);
+      to_mont(c.blami, lami, q, NS);
+      to_mont(c.blami2, BigUInt::mulmod(lami, lami, q), q, NS);
       K = HostF3Field{q, {one, pc, BigUInt()}};
       p->derived["basis_cubic"] = {s0, lam, pc};
     }
   }
   HostF3 xq = K.pow(x, q), xq2 = K.mul(xq, xq);
   for (int i = 0; i < 3; i++) {
-    to_mont(c.xpwr3[i], x3.c[i], q, kNS);
-    to_mont(c.xpwr4[i], x4.c[i], q, kNS);
-    to_mont(c.xpowq[i], xq.c[i], q, kNS);
-    to_mont(c.xpowq2[i], xq2.c[i], q, kNS);
+    to_mont(c.xpwr3[i], x3.c[i], q, NS);
+    to_mont(c.xpwr4[i], x4.c[i], q, NS);
+    to_mont(c.xpowq[i], xq.c[i], q, NS);
+    to_mont(c.xpowq2[i], xq2.c[i], q, NS);
   }
   BigUInt num = (q * q + one) - q, ph, rem;
   BigUInt::divmod(num, r, &ph, &rem);
@@ -691,6 +711,80 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
   p->derived["nqrinv2"] = {BigUInt::mulmod(vinv, vinv, q)};
   c.phibits = (uint32_t)ph.bits();
   return 0;
+}
+
+static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::string>& tab) {
+  BigUInt q, r, a, b, nqr, c0, c1, c2;
+  int k = 0;
+  if (!get_big(tab, "q", &q) || !get_big(tab, "r", &r) || !get_big(tab, "a", &a) || !get_big(tab, "b", &b) ||
+      !get_int(tab, "k", &k) || !get_big(tab, "nqr", &nqr) || !get_big(tab, "coeff0", &c0) ||
+      !get_big(tab, "coeff1", &c1) || !get_big(tab, "coeff2", &c2)) return 1;
+  if (k != 6) return fail("type d: only embedding degree 6 is on the GPU hot path (got k = %d)", k);
+  const bool wide = q.bits() >= 160 && q.bits() <= 255;
+  if (!wide && (q.bits() > 159 || q.bits() < 153))
+    return fail("type d: this build supports 153..159-bit q (20-byte coordinates) and 160..255-bit q (got %zu bits)", q.bits());
+  if (r.bits() > (wide ? 255u : 160u) || r.bits() < 3) return fail("type d: bad group order");
+  BigUInt hco(1);
+  auto ith = tab.find("h");
+  if (ith != tab.end()) BigUInt::from_dec(ith->second, &hco);
+  p->type = 'd';
+  p->full = false;
+  p->zr_len = (int)((r.bits() + 7) / 8);
+  if (!wide) {
+    memset(&p->zr, 0, sizeof p->zr);
+    r.to_words(p->zr.r, 5);
+    p->zr.zlen = (uint32_t)p->zr_len;
+    p->nlimbs = kNS;
+    p->g1_len = 2 * kWS; p->g2_len = 6 * kWS; p->gt_len = 6 * kWS;
+    fill_fp_consts(&p->fp, q, kNS);
+    fill_cc(&p->cc, a, b, r, q);
+    fill_hash(p, q, hco);                  // G1 cofactor = h (ecc/d_param.c:1016)
+    return fill_type_d<kNS>(p, p->d, q, r, a, b, nqr, c0, c1, c2);
+  }
+  const int NW = pbcb200_dw::kLimbs;
+  const int wb = (int)((q.bits() + 7) / 8);
+  p->dwide = true;
+  memset(&p->dw_zr, 0, sizeof p->dw_zr);
+  r.to_words(p->dw_zr.r, NW);
+  p->dw_zr.zlen = (uint32_t)p->zr_len;
+  p->nlimbs = NW;
+  p->g1_len = 2 * wb; p->g2_len = 6 * wb; p->gt_len = 6 * wb;
+  fill_fp_consts(&p->fp, q, NW);
+  fill_cc(&p->dw_cc, a, b, r, q);
+  fill_hash(p, q, hco);
+  memset(&p->dw_x, 0, sizeof p->dw_x);
+  p->dw_x.wb = (uint32_t)wb;
+  if (q.word(0) % 8 == 1) {
+    // Tonelli-Shanks (group_cc.cuh, fq_sqrt_ts): q - 1 = 2^s Q, exponent (Q - 1)/2, c = z^Q for the
+    // least non-residue z.  Any root serves: the kernels normalise its sign as the reference does.
+    BigUInt one(1), two(2), Q = q - one, z(2);
+    uint32_t s = 0;
+    while (!Q.bit(0)) { Q = Q / two; s++; }
+    const BigUInt qm1 = q - one, half = qm1 / two;
+    while (!(BigUInt::powmod(z, half, q) == qm1)) z = z + one;
+    HashConsts& h = p->hash;
+    BigUInt e = (Q - one) / two;
+    memset(h.exp, 0, sizeof h.exp);
+    e.to_words(h.exp, 16);
+    h.expbits = (uint32_t)e.bits();
+    h.sqrt_mode = 3;
+    p->hash_ok = h.cofbits <= 384;
+    p->dw_x.ts_s = s;
+    to_mont(p->dw_x.ts_c, BigUInt::powmod(z, Q, q), q, NW);
+    p->derived["sqrt_nonresidue"] = {z};
+  }
+#if PBC_CC_NAF
+  {
+    std::vector<int8_t> dg = naf_digits(r);
+    memset(&p->dw_naf, 0, sizeof p->dw_naf);
+    for (size_t i = 0; i < dg.size(); i++) {
+      if (dg[i]) p->dw_naf.nz[i >> 5] |= 1u << (i & 31);
+      if (dg[i] < 0) p->dw_naf.neg[i >> 5] |= 1u << (i & 31);
+    }
+    p->dw_naf.len = (uint32_t)dg.size();
+  }
+#endif
+  return fill_type_d<NW>(p, p->dw_d, q, r, a, b, nqr, c0, c1, c2);
 }
 
 // g_init_pairing (ecc/g_param.c:1248-1353), k = 10
@@ -855,6 +949,25 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
   }
   // make this handle's constants resident on the device
   std::lock_guard<std::mutex> lk(g_const_mu);
+  if (g_const_owner[dev] != p->id && p->dwide) {
+    CUDA_OK(cudaDeviceSynchronize());
+#if PBC_CC_NAF
+    const void* naf = &p->dw_naf;
+    const size_t naf_bytes = sizeof p->dw_naf;
+#else
+    const void* naf = nullptr;
+    const size_t naf_bytes = 0;
+#endif
+    pbcb200_dw::DWideConsts w = {&p->fp, &p->dw_cc, naf, &p->dw_d, &p->dw_zr, &p->hash, &p->dw_x,
+                                 sizeof p->fp, sizeof p->dw_cc, naf_bytes, sizeof p->dw_d, sizeof p->dw_zr,
+                                 sizeof p->hash, sizeof p->dw_x};
+    const int e = pbcb200_dw::dw_upload(w);
+    if (e == -2) return fail("type d: this build has no eight-limb instance (160..255-bit q)");
+    if (e < 0) return fail("type d: the constants of the eight-limb instance do not match its layout");
+    CUDA_OK((cudaError_t)e);
+    CUDA_OK(cudaDeviceSynchronize());
+    g_const_owner[dev] = p->id;
+  }
   if (g_const_owner[dev] != p->id) {
     CUDA_OK(cudaDeviceSynchronize());
     CUDA_OK(cudaMemcpyToSymbol(c_fp, &p->fp, sizeof(FpConsts)));
@@ -1057,8 +1170,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     return 0;
   }
   if (p->type == 'f' || p->type == 'd' || p->type == 'g') {
-    const bool isf = p->type == 'f', isg = p->type == 'g';
-    const size_t W = isf ? kF12Words : (isg ? kF10Words : kF6DWords);
+    const bool isf = p->type == 'f', isg = p->type == 'g', wide = p->dwide;
+    const size_t W = isf ? kF12Words : (isg ? kF10Words : 6 * (size_t)p->nlimbs);
     size_t m = job.mode == kProd ? n * job.k : n;
     uint32_t* mv = (uint32_t*)ws;                // [W][m]
     uint32_t* flag = mv + W * m;                 // [m]
@@ -1074,13 +1187,15 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       if (job.pp_tab) tab = (const uint32_t*)job.pp_tab;
       else {
         uint32_t* t = (uint32_t*)((uint8_t*)ws + ws_bytes(p, job, n) - cc_table_bytes(p));
-        if (isg) k_cc_pp_init<kWG><<<1, 32, 0, st>>>(d_in1, t, rows);
+        if (wide) pbcb200_dw::dw_pp_init(d_in1, t, rows, st);
+        else if (isg) k_cc_pp_init<kWG><<<1, 32, 0, st>>>(d_in1, t, rows);
         else k_cc_pp_init<kWS><<<1, 32, 0, st>>>(d_in1, t, rows);
         LAUNCHED();
         tab = t;
       }
     }
-    if (isf && PBC_F_SLOTS && p->f.slots_ok) {
+    if (wide) pbcb200_dw::dw_miller(d_in1, d_in2, mv, flag, m, stride1, tab, rows, st);
+    else if (isf && PBC_F_SLOTS && p->f.slots_ok) {
       uint32_t* gq = mv + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0);   // after the Miller values and flags
       k_f_miller_s<kBlockFSM><<<(unsigned)((m + kBlockFSM - 1) / kBlockFSM), kBlockFSM, kSmemFMillerS, st>>>(d_in1, d_in2, mv, flag, gq, m, stride1, tab, rows);
     } else if (isf) k_f_miller<kBlockCCMiller><<<gm, kBlockCCMiller, 0, st>>>(d_in1, d_in2, mv, flag, m, stride1, tab, rows);
@@ -1092,7 +1207,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       uint32_t* mvo = flag + m;                  // [W][n]
       uint32_t* flago = mvo + W * n;
       unsigned gp = (unsigned)((n + kBlockCC - 1) / kBlockCC);
-      if (isf) k_f_prod<kBlockCC><<<gp, kBlockCC, 0, st>>>(mv, flag, mvo, flago, job.k, n, m);
+      if (wide) pbcb200_dw::dw_prod(mv, flag, mvo, flago, job.k, n, m, st);
+      else if (isf) k_f_prod<kBlockCC><<<gp, kBlockCC, 0, st>>>(mv, flag, mvo, flago, job.k, n, m);
       else if (isg) k_g_prod<kBlockCC><<<gp, kBlockCC, 0, st>>>(mv, flag, mvo, flago, job.k, n, m);
       else k_d_prod<kBlockCC><<<gp, kBlockCC, 0, st>>>(mv, flag, mvo, flago, job.k, n, m);
       LAUNCHED();
@@ -1101,7 +1217,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     STAGE(2);
     unsigned gf = (unsigned)((n + kBlockCC - 1) / kBlockCC);
     unsigned gfm = (unsigned)((n + kBlockCCMiller - 1) / kBlockCCMiller);
-    if (isf && PBC_F_SLOTS && p->f.slots_ok && p->f.bn) {
+    if (wide) pbcb200_dw::dw_finalexp(mv, flag, d_out, n, st);
+    else if (isf && PBC_F_SLOTS && p->f.slots_ok && p->f.bn) {
       uint32_t* stash = (uint32_t*)ws + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0) + (size_t)kFGWords * m;
       k_f_finalexp_s<kBlockFS><<<(unsigned)((n + kBlockFS - 1) / kBlockFS), kBlockFS, kSmemFFinalS, st>>>(mv, flag, d_out, stash, n);
     } else if (isf) k_f_finalexp<kBlockCCMiller><<<gfm, kBlockCCMiller, 0, st>>>(mv, flag, d_out, n);
@@ -1361,7 +1478,8 @@ int pbc_b200_pp_init(pbc_b200_pairing_t* p, pbc_b200_pp_t** out, const unsigned 
   if (e == cudaSuccess && p->type == 'a') { k_a_pp_init<32><<<1, 32, kSmemAPPInit, st>>>(pp->d_in1, (uint32_t*)pp->d_tab); LAUNCHED(); }
   if (e == cudaSuccess && p->type == '1') { k_a1_pp_init<32><<<1, 32, kSmemA1PPInit, st>>>(pp->d_in1, (uint32_t*)pp->d_tab, p->a1_rows); LAUNCHED(); }
   if (e == cudaSuccess && cc) {
-    if (p->type == 'g') k_cc_pp_init<kWG><<<1, 32, 0, st>>>(pp->d_in1, (uint32_t*)pp->d_tab, cc_table_rows(p));
+    if (p->dwide) pbcb200_dw::dw_pp_init(pp->d_in1, (uint32_t*)pp->d_tab, cc_table_rows(p), st);
+    else if (p->type == 'g') k_cc_pp_init<kWG><<<1, 32, 0, st>>>(pp->d_in1, (uint32_t*)pp->d_tab, cc_table_rows(p));
     else k_cc_pp_init<kWS><<<1, 32, 0, st>>>(pp->d_in1, (uint32_t*)pp->d_tab, cc_table_rows(p));
     LAUNCHED();
   }
@@ -1446,6 +1564,7 @@ void pbc_b200_host_free(void* ptr) { if (ptr) cudaFreeHost(ptr); }
 static double bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters, int reps, size_t smem) {
   if (!p) { fail("null argument"); return -1; }
   if (p->type == '1') { fail("bench_fpmul: not built for type a1"); return -1; }
+  if (p->dwide) { fail("bench_fpmul: not built for the eight-limb type d field"); return -1; }
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || ctx_prepare(p, dev)) return -1;
   const int threads = 128;
@@ -1600,7 +1719,8 @@ static int enqueue_group(pbc_b200_pairing_s* p, int which /*0 = G1, 1 = GT, 2 = 
   } else {
     unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
     const bool isg = p->type == 'g';
-    if (which == 0 && isg) k_cc_g1_mul<kBlockCC, kWG><<<g, kBlockCC, 0, st>>>(d_in, d_k, d_out, n);
+    if (p->dwide) pbcb200_dw::dw_group(which, d_out, d_in, d_k, n, st);
+    else if (which == 0 && isg) k_cc_g1_mul<kBlockCC, kWG><<<g, kBlockCC, 0, st>>>(d_in, d_k, d_out, n);
     else if (which == 0) k_cc_g1_mul<kBlockCC, kWS><<<g, kBlockCC, 0, st>>>(d_in, d_k, d_out, n);
     else if (which == 2 && isg) k_cc_g2_mul<KF5, kBlockCC><<<g, kBlockCC, 0, st>>>(d_in, d_k, d_out, n);
     else if (which == 1 && isg) k_g_gt_pow<kBlockCC><<<g, kBlockCC, 0, st>>>(d_in, d_k, d_out, n);
@@ -1687,7 +1807,7 @@ int pbc_b200_gt_pow_zn_device(pbc_b200_pairing_t* p, void* d_out, const void* d_
 static int run_from_hash(pbc_b200_pairing_s* p, unsigned char* out, const unsigned char* data, size_t len, size_t n,
                          bool device, void* stream) {
   if (!p || (n && (!out || !data))) return fail("null argument");
-  if (p->type != '1' && !p->hash_ok) return fail("element_from_hash: needs q = 3 mod 4 or q = 5 mod 8 and a cofactor below 2^384");
+  if (p->type != '1' && !p->hash_ok) return fail("element_from_hash: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q) and a cofactor below 2^384");
   if (len == 0 || len > (1u << 20)) return fail("element_from_hash: hash length must be 1..2^20 bytes");
   if (n == 0) return 0;
   std::lock_guard<std::mutex> lk(p->mu);
@@ -1743,7 +1863,8 @@ static int run_from_hash(pbc_b200_pairing_s* p, unsigned char* out, const unsign
     LAUNCHED();
   } else {
     unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
-    if (p->type == 'g') k_cc_g1_from_hash<kBlockCC, kWG><<<g, kBlockCC, 0, st>>>(d_data, (int)len, d_out, n);
+    if (p->dwide) pbcb200_dw::dw_from_hash(d_data, (int)len, d_out, n, st);
+    else if (p->type == 'g') k_cc_g1_from_hash<kBlockCC, kWG><<<g, kBlockCC, 0, st>>>(d_data, (int)len, d_out, n);
     else k_cc_g1_from_hash<kBlockCC, kWS><<<g, kBlockCC, 0, st>>>(d_data, (int)len, d_out, n);
     LAUNCHED();
   }
@@ -1772,7 +1893,7 @@ extern "C" int pbc_b200_pairing_length_in_bytes_compressed_G1(const pbc_b200_pai
 extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in,
                                                  size_t n) {
   if (!p || (n && (!out || !in))) return fail("null argument");
-  if (p->type != '1' && !p->hash_ok) return fail("element_from_bytes_compressed: needs q = 3 mod 4 or q = 5 mod 8");
+  if (p->type != '1' && !p->hash_ok) return fail("element_from_bytes_compressed: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q)");
   if (n == 0) return 0;
   std::lock_guard<std::mutex> lk(p->mu);
   int dev = 0;
@@ -1801,7 +1922,8 @@ extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned
     k_a_g1_decompress<kBlockMiller><<<g, kBlockMiller, (size_t)5 * 64 * kBlockMiller, st>>>(d_in, d_out, n);
   } else {
     unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
-    if (p->type == 'g') k_cc_g1_decompress<kBlockCC, kWG><<<g, kBlockCC, 0, st>>>(d_in, d_out, n);
+    if (p->dwide) pbcb200_dw::dw_decompress(d_in, d_out, n, st);
+    else if (p->type == 'g') k_cc_g1_decompress<kBlockCC, kWG><<<g, kBlockCC, 0, st>>>(d_in, d_out, n);
     else k_cc_g1_decompress<kBlockCC, kWS><<<g, kBlockCC, 0, st>>>(d_in, d_out, n);
   }
   LAUNCHED();
@@ -1829,7 +1951,8 @@ static int enqueue_gt_mul(pbc_b200_pairing_s* p, uint8_t* d_out, const uint8_t* 
     k_a1_gt_mul<kBlockA1G><<<g, kBlockA1G, (size_t)7 * kSlotA1 * kBlockA1G, st>>>(d_a, d_b, d_out, n);
   } else {
     unsigned g = (unsigned)((n + 63) / 64);
-    if (p->type == 'f') k_f_tower_op<<<g, 64, 0, st>>>(0, d_out, d_a, d_b, n);
+    if (p->dwide) pbcb200_dw::dw_tower_op(0, d_out, d_a, d_b, n, st);
+    else if (p->type == 'f') k_f_tower_op<<<g, 64, 0, st>>>(0, d_out, d_a, d_b, n);
     else if (p->type == 'g') k_g_tower_op<<<g, 64, 0, st>>>(0, d_out, d_a, d_b, n);
     else k_d_tower_op<<<g, 64, 0, st>>>(0, d_out, d_a, d_b, n);
   }
@@ -1907,7 +2030,7 @@ extern "C" int pbc_b200_is_almost_coddh(pbc_b200_pairing_t* p, unsigned char* fl
   if (enqueue_pairings(p, job, t0.as<uint8_t>(), da.as<uint8_t>(), dd.as<uint8_t>(), n, ws.p, st)) return 1;
   if (enqueue_pairings(p, job, t1.as<uint8_t>(), db.as<uint8_t>(), dc.as<uint8_t>(), n, ws.p, st)) return 1;
   if (enqueue_gt_mul(p, t2.as<uint8_t>(), t0.as<uint8_t>(), t1.as<uint8_t>(), n, st)) return 1;
-  size_t wb = p->type == '1' ? (size_t)p->gt_len / 2 : (p->type == 'a' ? (size_t)kWA : (p->type == 'g' ? (size_t)kWG : (size_t)kWS));
+  size_t wb = p->type == '1' ? (size_t)p->gt_len / 2 : (p->type == 'a' ? (size_t)kWA : (p->type == 'g' ? (size_t)kWG : (size_t)p->g1_len / 2));
   k_coddh_flags<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(df.as<uint8_t>(), t0.as<uint8_t>(), t1.as<uint8_t>(),
                                                             t2.as<uint8_t>(), lt, wb, n);
   LAUNCHED();
@@ -2027,6 +2150,8 @@ extern "C" int pbc_b200_fp_op(pbc_b200_pairing_t* p, int op, unsigned char* out,
   } else if (p->type == 'a') {
     CUDA_OK(allow_smem(k_fp_op<kNA, true, 64, 128>, 4 * 64 * 128));
     k_fp_op<kNA, true, 64, 128><<<g, 128, 4 * 64 * 128>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
+  } else if (p->dwide) {
+    pbcb200_dw::dw_fq_op(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n, 0);
   } else if (p->type == 'g') {
     k_fq_op<kWG><<<g, 128>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
   } else {
@@ -2056,7 +2181,8 @@ extern "C" int pbc_b200_tower_op(pbc_b200_pairing_t* p, int op, unsigned char* o
   CUDA_OK(cudaMemcpy(da.p, a, n * wb, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(db.p, b ? b : a, n * wb, cudaMemcpyHostToDevice));
   unsigned g = (unsigned)((n + 63) / 64);
-  if (p->type == 'f') k_f_tower_op<<<g, 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
+  if (p->dwide) pbcb200_dw::dw_tower_op(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n, 0);
+  else if (p->type == 'f') k_f_tower_op<<<g, 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
   else if (p->type == 'g') k_g_tower_op<<<g, 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
   else k_d_tower_op<<<g, 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
   LAUNCHED();

@@ -18,11 +18,38 @@ namespace pbcb200 {
 // PBC_NS: 32-bit limbs of the small field.  5 = minimal (product-scanning multiplier, 55 products,
 // ~140 instructions); 6 = one spare limb so the even/odd operand-scanning multiplier of fp.cuh applies
 // (78 products but ~105 instructions) -- an A/B experiment, see DESIGN.md.
+// PBC_FQ_WIDE = 1: the eight-limb instance of type D for 160- to 255-bit q (engine_d_wide.cu, its own
+// translation unit and namespace): the wire width is a run-time constant there, and q = 1 mod 8 takes
+// Tonelli-Shanks square roots.
+#ifndef PBC_FQ_WIDE
+#define PBC_FQ_WIDE 0
+#endif
 #ifndef PBC_NS
 #define PBC_NS 5
 #endif
 constexpr int kNS = PBC_NS;    // 32-bit limbs
+#if !PBC_FQ_WIDE
 constexpr int kWS = 20;        // wire bytes per coordinate (arith/montfp.c:577)
+__device__ __forceinline__ int fq_wb() { return kWS; }
+#endif
+
+// constants of the wide instance only: the wire width ceil(bits(q)/8) and, for q = 1 mod 8, the
+// Tonelli-Shanks data (q - 1 = 2^s Q with Q odd, c = z^Q for a quadratic non-residue z, Montgomery form;
+// the exponent (Q - 1)/2 sits in HashConsts::exp)
+template <int NS>
+struct FqWideConstsT {
+  uint32_t wb;
+  uint32_t ts_s;
+  uint32_t pad[2];
+  uint32_t ts_c[NS];
+};
+#if PBC_FQ_WIDE
+__constant__ FqWideConstsT<kNS> c_fqx;
+__device__ __forceinline__ int fq_wb() { return (int)c_fqx.wb; }
+#endif
+// coordinate width of the width-generic kernels: W, or for W = 0 the run-time width of the wide instance
+template <int W>
+__device__ __forceinline__ int wire_w() { return W ? W : fq_wb(); }
 
 struct Fq { uint32_t v[kNS]; };
 
@@ -42,14 +69,14 @@ __device__ __forceinline__ void fq_mul_os(Fq& r, const Fq& a, const Fq& b);
 #if PBC_FQ_CALL
 __device__ __noinline__ Fq fq_mul_call(Fq a, Fq b) {
   Fq r;
-  if (kNS % 2 == 0) mont_mul<kNS + (kNS & 1), false>(r.v, a.v, b.v);
+  if constexpr (kNS % 2 == 0) mont_mul<kNS + (kNS & 1), false>(r.v, a.v, b.v);
   else if (PBC_FQ_CALL_OS) fq_mul_os(r, a, b);
   else mont_mul_ps<kNS, false>(r.v, a.v, b.v);
   return r;
 }
 __device__ __noinline__ Fq fq_sqr_call(Fq a) {
   Fq r;
-  if (kNS % 2 == 0) mont_mul<kNS + (kNS & 1), false>(r.v, a.v, a.v);
+  if constexpr (kNS % 2 == 0) mont_mul<kNS + (kNS & 1), false>(r.v, a.v, a.v);
   else if (PBC_FQ_CALL_OS >= 2) fq_mul_os(r, a, a);
   else mont_sqr_ps<kNS, false>(r.v, a.v);
   return r;
@@ -209,6 +236,7 @@ __device__ __forceinline__ void fqw_sub(FqW& r, const FqW& a, const FqW& b) {
 #define PBC_MULW_PAIR(lo, hi, x, y) PBC_ASM("mul.lo.u32 %0, %2, %3; mul.hi.u32 %1, %2, %3;" : "=r"(lo), "=r"(hi) : "r"(x), "r"(y))
 #endif
 #define PBC_CARRY_TO(w) PBC_ASM("addc.u32 %0, 0, 0;" : "=r"(w))
+#if PBC_NS == 5
 __device__ __forceinline__ void fqw_mul(FqW& t, const Fq& a, const Fq& b) {
   static_assert(kNS == 5, "the row schedule below is written out for five limbs");
 #if PBC_FQW_OS
@@ -271,6 +299,10 @@ __device__ __forceinline__ void fqw_mul(FqW& t, const Fq& a, const Fq& b) {
   t.v[2 * kNS - 1] = u0;
 #endif
 }
+#else
+// any even limb count (the wide instance): the operand-scanning double-width product of fp.cuh
+__device__ __forceinline__ void fqw_mul(FqW& t, const Fq& a, const Fq& b) { mul_wide<kNS>(t.v, a.v, b.v); }
+#endif
 // Montgomery reduction of t < 2 q R to the canonical residue (two conditional subtractions)
 __device__ __forceinline__ void fqw_redc2(Fq& r, const FqW& t) {
   uint32_t m[kNS], o[kNS];
@@ -413,6 +445,7 @@ struct FqAcc { uint32_t E[10], O[10], K[5]; };
 
 // c = a b (the schedule of fqw_mul: every word of E and O is written, fresh words take the carries); K is
 // NOT written: the first fqa_mac after it sets K (SETK), a lone product is merged with fqa_merge<false>.
+#if PBC_NS == 5
 __device__ __forceinline__ void fqa_mul(FqAcc& c, const Fq& a, const Fq& b) {
   static_assert(kNS == 5, "the row schedule below is written out for five limbs");
   uint32_t* E = c.E;
@@ -453,6 +486,7 @@ __device__ __forceinline__ void fqa_mul(FqAcc& c, const Fq& a, const Fq& b) {
   PBC_MADW_NEXT(O[7], O[8], x[3], y[4]);
   PBC_CARRY_TO(O[9]);
 }
+#endif
 // c += a b.  SETK: the first accumulation after fqa_mul -- the first capture at each word writes K.
 // (K[i+1] is first touched by row i's long run, K[0] by row 0's short run.)
 template <bool SETK>
@@ -499,6 +533,7 @@ __device__ __forceinline__ void fqa_merge(FqW& t, const FqAcc& c) {
 // the word above it, which the next row's top pair takes as its addend.  r = X + t_hi - {0, q, 2q}.
 // 25 IMAD.WIDE + 5 IMAD and about 30 additions; the column-wise fqw_redc2 needs about 60 and a serial
 // chain of three-word column sums.
+#if PBC_NS == 5
 template <bool TWO>
 __device__ __forceinline__ void fqw_redc_os(Fq& r, const FqW& t) {
   static_assert(kNS == 5, "written out for five limbs");
@@ -570,7 +605,25 @@ __device__ __forceinline__ void fq_mul_os(Fq& r, const Fq& a, const Fq& b) {
   fqa_merge<false>(t, c);
   fqw_redc_os<false>(r, t);
 }
+#else
+// any even limb count (the wide instance): redc_wide of fp.cuh, which takes t < 2 q R and returns the
+// canonical residue (two conditional subtractions), so TWO makes no difference
+template <bool TWO>
+__device__ __forceinline__ void fqw_redc_os(Fq& r, const FqW& t) {
+  uint32_t w[2 * kNS + 1];
+#pragma unroll
+  for (int k = 0; k < 2 * kNS; k++) w[k] = t.v[k];
+  w[2 * kNS] = 0;
+  redc_wide<kNS>(r.v, w);
+}
+__device__ __forceinline__ void fq_mul_os(Fq& r, const Fq& a, const Fq& b) {
+  FqW t;
+  fqw_mul(t, a, b);
+  fqw_redc_os<false>(r, t);
+}
+#endif
 
+#if !PBC_FQ_WIDE
 // wire bytes (big-endian, 20 per coordinate) -> Montgomery form (arith/montfp.c:498-517 reduces mod q)
 __device__ __forceinline__ void fq_from_wire(Fq& r, const uint8_t* p) {
   limbs_from_be<kNS, kWS>(r.v, p);
@@ -582,10 +635,44 @@ __device__ __forceinline__ void fq_to_wire(uint8_t* p, const Fq& a) {
   mont_mul_ps<kNS, false>(x, a.v, one);
   limbs_to_be<kNS, kWS>(p, x);
 }
+#else
+// the wide instance: ceil(bits(q)/8) bytes per coordinate, a run-time constant, read and written byte
+// by byte (no alignment).  Any wb-byte value is below 2^256 = R, and mont_mul_ps reduces a R q-bounded
+// product to the canonical residue (a < R, b < q, q < R/2), as arith/montfp.c:498-517 reduces mod q.
+__device__ __forceinline__ void fq_from_wire(Fq& r, const uint8_t* p) {
+  const int wb = fq_wb();
+#pragma unroll
+  for (int k = 0; k < kNS; k++) {
+    uint32_t w = 0;
+#pragma unroll
+    for (int b = 0; b < 4; b++) {
+      int pos = wb - 1 - (4 * k + b);
+      if (pos >= 0) w |= (uint32_t)p[pos] << (8 * b);
+    }
+    r.v[k] = w;
+  }
+  mont_mul_ps<kNS, false>(r.v, r.v, c_fp.r2);
+}
+__device__ __forceinline__ void fq_to_wire(uint8_t* p, const Fq& a) {
+  const int wb = fq_wb();
+  uint32_t one[kNS] = {1}, x[kNS];
+  mont_mul_ps<kNS, false>(x, a.v, one);
+#pragma unroll
+  for (int k = 0; k < kNS; k++) {
+#pragma unroll
+    for (int b = 0; b < 4; b++) {
+      int pos = wb - 1 - (4 * k + b);
+      if (pos >= 0) p[pos] = (uint8_t)(x[k] >> (8 * b));
+    }
+  }
+}
+#endif
 
 // the same for a coordinate width that is not a multiple of four bytes (g149: 19), byte by byte
 template <int WB>
 __device__ __forceinline__ void fq_from_wire_b(Fq& r, const uint8_t* p) {
+  if constexpr (WB == 0) fq_from_wire(r, p);         // the run-time width of the wide instance
+  else {
 #pragma unroll
   for (int k = 0; k < kNS; k++) {
     uint32_t w = 0;
@@ -597,6 +684,7 @@ __device__ __forceinline__ void fq_from_wire_b(Fq& r, const uint8_t* p) {
     r.v[k] = w;
   }
   mont_mul_ps<kNS, false>(r.v, r.v, c_fp.r2);
+  }
 }
 template <int WB>
 __device__ __forceinline__ void fq_to_wire_b(uint8_t* p, const Fq& a) {
@@ -609,15 +697,18 @@ __device__ __forceinline__ void fq_to_wire_b(uint8_t* p, const Fq& a) {
   }
 }
 
-// width-generic front ends: the word-wise path when the width allows it, else byte by byte
+// width-generic front ends: the word-wise path when the width allows it, else byte by byte; WB = 0: the
+// run-time width of the wide instance
 template <int WB>
 __device__ __forceinline__ void fq_from_wire_w(Fq& r, const uint8_t* p) {
-  if constexpr (WB % 4 == 0) { limbs_from_be<kNS, WB>(r.v, p); mont_mul_ps<kNS, false>(r.v, r.v, c_fp.r2); }
+  if constexpr (WB == 0) fq_from_wire(r, p);
+  else if constexpr (WB % 4 == 0) { limbs_from_be<kNS, WB>(r.v, p); mont_mul_ps<kNS, false>(r.v, r.v, c_fp.r2); }
   else fq_from_wire_b<WB>(r, p);
 }
 template <int WB>
 __device__ __forceinline__ void fq_to_wire_w(uint8_t* p, const Fq& a) {
-  if constexpr (WB % 4 == 0) { uint32_t one[kNS] = {1}, x[kNS]; mont_mul_ps<kNS, false>(x, a.v, one); limbs_to_be<kNS, WB>(p, x); }
+  if constexpr (WB == 0) fq_to_wire(p, a);
+  else if constexpr (WB % 4 == 0) { uint32_t one[kNS] = {1}, x[kNS]; mont_mul_ps<kNS, false>(x, a.v, one); limbs_to_be<kNS, WB>(p, x); }
   else fq_to_wire_b<WB>(p, a);
 }
 

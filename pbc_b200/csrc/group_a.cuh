@@ -14,11 +14,19 @@
 
 namespace pbcb200 {
 
-struct ZrConsts {
-  uint32_t r[5];         // group order, little-endian words (every supported type has r < 2^160)
+// words of a scalar: 5 (every type of engine.cu has r < 2^160), 8 in the wide type D instance
+// (engine_d_wide.cu: r < 2^256)
+#ifndef PBC_ZR_WORDS
+#define PBC_ZR_WORDS 5
+#endif
+constexpr int kZW = PBC_ZR_WORDS;
+template <int NW>
+struct ZrConstsT {
+  uint32_t r[NW];        // group order, little-endian words
   uint32_t zlen;         // Zr wire bytes: ceil(bits(r)/8) (20 for a, f, d159; 19 for g149)
   uint32_t pad[2];
 };
+typedef ZrConstsT<kZW> ZrConsts;
 __constant__ ZrConsts c_zr;
 
 // element_from_hash on G1 (ecc/curve.c:455-482): square-root exponent and cofactor, plain integers
@@ -79,7 +87,7 @@ constexpr int kWZ = 20;  // Zr wire bytes of a.param, f.param, d159.param (c_zr.
 __device__ __forceinline__ void zr_from_wire(uint32_t* k, const uint8_t* p) {
   const int zlen = (int)c_zr.zlen;
 #pragma unroll
-  for (int i = 0; i < 5; i++) {
+  for (int i = 0; i < kZW; i++) {
     uint32_t w = 0;
 #pragma unroll
     for (int b = 0; b < 4; b++) {
@@ -89,18 +97,18 @@ __device__ __forceinline__ void zr_from_wire(uint32_t* k, const uint8_t* p) {
     k[i] = w;
   }
   for (int it = 0; it < 4096; it++) {
-    uint32_t d[5], borrow;
+    uint32_t d[kZW], borrow;
     PBC_ASM("sub.cc.u32 %0, %1, %2;" : "=r"(d[0]) : "r"(k[0]), "r"(c_zr.r[0]));
 #pragma unroll
-    for (int i = 1; i < 5; i++) PBC_ASM("subc.cc.u32 %0, %1, %2;" : "=r"(d[i]) : "r"(k[i]), "r"(c_zr.r[i]));
+    for (int i = 1; i < kZW; i++) PBC_ASM("subc.cc.u32 %0, %1, %2;" : "=r"(d[i]) : "r"(k[i]), "r"(c_zr.r[i]));
     PBC_ASM("subc.u32 %0, 0, 0;" : "=r"(borrow));
     if (borrow) break;
 #pragma unroll
-    for (int i = 0; i < 5; i++) k[i] = d[i];
+    for (int i = 0; i < kZW; i++) k[i] = d[i];
   }
 }
 __device__ __forceinline__ int zr_top_bit(const uint32_t* k) {
-  for (int j = 159; j >= 0; j--)
+  for (int j = 32 * kZW - 1; j >= 0; j--)
     if ((k[j >> 5] >> (j & 31)) & 1u) return j;
   return -1;
 }

@@ -10,8 +10,10 @@
 #pragma once
 #include "group_a.cuh"
 #include "pairing_d.cuh"
+#if !PBC_FQ_WIDE
 #include "pairing_f.cuh"
 #include "pairing_g.cuh"
+#endif
 
 namespace pbcb200 {
 
@@ -23,10 +25,10 @@ k_cc_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
   Fq xP, yP, X, Y, Z, Z2, M, Y2, t, u, H, R;
-  fq_from_wire_w<W>(xP, P + idx * (2 * W));
-  fq_from_wire_w<W>(yP, P + idx * (2 * W) + W);
+  fq_from_wire_w<W>(xP, P + idx * (2 * wire_w<W>()));
+  fq_from_wire_w<W>(yP, P + idx * (2 * wire_w<W>()) + wire_w<W>());
   bool ok = cc_on_curve(xP, yP);
-  uint32_t k[5];
+  uint32_t k[kZW];
   zr_from_wire(k, K + idx * c_zr.zlen);
   int top = zr_top_bit(k);
   X = xP;
@@ -89,9 +91,44 @@ k_cc_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   fq_mul(u, u, t);
   fq_mul(Y, Y, u);
   if (inf) { fq_zero(X); fq_zero(Y); }
-  fq_to_wire_w<W>(out + idx * (2 * W), X);
-  fq_to_wire_w<W>(out + idx * (2 * W) + W, Y);
+  fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()), X);
+  fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()) + wire_w<W>(), Y);
 }
+
+#if PBC_FQ_WIDE
+// Tonelli-Shanks (q = 1 mod 8, the wide instance; HashConsts::sqrt_mode 3):  q - 1 = 2^s Q, Q odd,
+// x = t^((Q-1)/2), y = t x, b = y x = t^Q, c = z^Q (z a non-residue).  While b != 1: the least i with
+// b^(2^i) = 1 (none below m: t is not a square, y is left as it is and fails the caller's y^2 == t),
+// w = c^(2^(m-i-1)), y = y w, c = w^2, b = b c, m = i.  y is then a root of t; which of the two does not
+// matter, the callers normalise its sign as the reference does (ecc/curve.c).
+__device__ __noinline__ void fq_sqrt_ts(Fq* out, const Fq* tp) {
+  Fq t = *tp, x, y, b, c, w, one;
+  fq_one(one);
+  x = t;
+  for (int j = (int)c_hash.expbits - 2; j >= 0; j--) {
+    fq_sqr(x, x);
+    if ((c_hash.exp[j >> 5] >> (j & 31)) & 1u) fq_mul(x, x, t);
+  }
+  if (c_hash.expbits == 0) x = one;
+  fq_mul(y, t, x);
+  fq_mul(b, y, x);
+  fq_set(c, c_fqx.ts_c);
+  int m = (int)c_fqx.ts_s;
+  for (int it = 0; it < 64 && !fq_eq(b, one); it++) {
+    int i = 1;
+    fq_sqr(w, b);
+    while (i < m && !fq_eq(w, one)) { fq_sqr(w, w); i++; }
+    if (i >= m) break;
+    w = c;
+    for (int j = 0; j < m - i - 1; j++) fq_sqr(w, w);
+    fq_mul(y, y, w);
+    fq_sqr(c, w);
+    fq_mul(b, b, c);
+    m = i;
+  }
+  *out = y;
+}
+#endif
 
 // element_from_hash on G1 for the five-limb fields (ecc/curve.c:455-482): try-and-increment, the odd
 // square root (q = 3 mod 4: t^((q+1)/4); q = 5 mod 8: Atkin's b = (2t)^((q-5)/8), i = 2 t b^2,
@@ -115,6 +152,16 @@ k_cc_g1_from_hash(const uint8_t* __restrict__ data, int len, uint8_t* __restrict
     fq_add(t, t, A);
     fq_mul(t, t, x);
     fq_add(t, t, B);                       // t = x^3 + A x + B
+#if PBC_FQ_WIDE
+    if (c_hash.sqrt_mode == 3) {
+      fq_sqrt_ts(&y, &t);
+      fq_sqr(w, y);
+      if (fq_eq(w, t)) break;
+      fq_sqr(x, x);
+      fq_add(x, x, one);
+      continue;
+    }
+#endif
     if (c_hash.sqrt_mode == 1) u = t; else fq_dbl(u, t);
     b = u;
     for (int j = (int)c_hash.expbits - 2; j >= 0; j--) {
@@ -142,8 +189,8 @@ k_cc_g1_from_hash(const uint8_t* __restrict__ data, int len, uint8_t* __restrict
     if (!(c[0] & 1u) && !fp_is_zero<kNS>(c)) fq_neg(y, y);
   }
   if (c_hash.cofbits <= 1) {               // cofactor 1: the point itself
-    fq_to_wire_w<W>(out + idx * (2 * W), x);
-    fq_to_wire_w<W>(out + idx * (2 * W) + W, y);
+    fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()), x);
+    fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()) + wire_w<W>(), y);
     return;
   }
   X = x;
@@ -203,8 +250,8 @@ k_cc_g1_from_hash(const uint8_t* __restrict__ data, int len, uint8_t* __restrict
   fq_mul(u, u, t);
   fq_mul(Y, Y, u);
   if (inf) { fq_zero(X); fq_zero(Y); }
-  fq_to_wire_w<W>(out + idx * (2 * W), X);
-  fq_to_wire_w<W>(out + idx * (2 * W) + W, Y);
+  fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()), X);
+  fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()) + wire_w<W>(), Y);
 }
 
 // element_from_bytes_compressed on G1 for the five-limb fields (ecc/curve.c:799-813): x (20 bytes) ||
@@ -214,7 +261,7 @@ __global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
 k_cc_g1_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
-  const uint8_t* p = in + idx * (W + 1);
+  const uint8_t* p = in + idx * (wire_w<W>() + 1);
   Fq x, y, t, b, u, w, one, k;
   fq_from_wire_b<W>(x, p);             // items are W + 1 bytes apart: byte loads
   fq_one(one);
@@ -224,6 +271,9 @@ k_cc_g1_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, si
   fq_mul(t, t, x);
   fq_set(k, c_cc.B);
   fq_add(t, t, k);
+#if PBC_FQ_WIDE
+  if (c_hash.sqrt_mode == 3) fq_sqrt_ts(&y, &t); else {
+#endif
   if (c_hash.sqrt_mode == 1) u = t; else fq_dbl(u, t);
   b = u;
   for (int j = (int)c_hash.expbits - 2; j >= 0; j--) {
@@ -240,15 +290,18 @@ k_cc_g1_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, si
     fq_mul(y, t, b);
     fq_mul(y, y, w);
   }
+#if PBC_FQ_WIDE
+  }
+#endif
   fq_sqr(w, y);
   bool ok = fq_eq(w, t);
   uint32_t c[kNS], o1[kNS] = {1};
   mont_mul_ps<kNS, false>(c, y.v, o1);
-  bool odd = (c[0] & 1u) != 0, want_odd = p[W] != 0;
+  bool odd = (c[0] & 1u) != 0, want_odd = p[wire_w<W>()] != 0;
   if (odd != want_odd && !fp_is_zero<kNS>(c)) fq_neg(y, y);
   if (!ok) { fq_zero(x); fq_zero(y); }
-  fq_to_wire_w<W>(out + idx * (2 * W), x);
-  fq_to_wire_w<W>(out + idx * (2 * W) + W, y);
+  fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()), x);
+  fq_to_wire_w<W>(out + idx * (2 * wire_w<W>()) + wire_w<W>(), y);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -256,9 +309,10 @@ k_cc_g1_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, si
 // field: struct El; mul/sqr/inv on pointers (the tower's out-of-line routines), add/sub/dbl inline,
 // wire <-> basis-in-use conversion, and the curve constants.
 // ---------------------------------------------------------------------------------------------
+#if !PBC_FQ_WIDE
 struct KF2 {                       // type f
   typedef F2 El;
-  static constexpr int kWire = 2 * kWS;
+  static __device__ __forceinline__ int wire() { return 2 * kWS; }
   static __device__ __forceinline__ void mul(El* r, const El* a, const El* b) { f2_mul(r, a, b); }
   static __device__ __forceinline__ void sqr(El* r, const El* a) { f2_sqr(r, a); }
   static __device__ __forceinline__ void inv(El* r, const El* a) { f2_inv(r, a); }
@@ -290,9 +344,10 @@ struct KF2 {                       // type f
     fq_to_wire(p + kWS, o.b);
   }
 };
+#endif
 struct KF3 {                       // type d
   typedef F3 El;
-  static constexpr int kWire = 3 * kWS;
+  static __device__ __forceinline__ int wire() { return 3 * fq_wb(); }
   static __device__ __forceinline__ void mul(El* r, const El* a, const El* b) { f3_mul(r, a, b); }
   static __device__ __forceinline__ void sqr(El* r, const El* a) { f3_sqr(r, a); }
   static __device__ __forceinline__ void inv(El* r, const El* a) { f3_inv(r, a); }
@@ -307,7 +362,7 @@ struct KF3 {                       // type d
   static __device__ __forceinline__ void add_curve_b(El& r) { Fq k; fq_set(k, c_d.twist_b); fq_add(r.c[0], r.c[0], k); }
   static __device__ __forceinline__ void from_wire(El& r, const uint8_t* p) {
 #pragma unroll
-    for (int i = 0; i < 3; i++) fq_from_wire(r.c[i], p + i * kWS);
+    for (int i = 0; i < 3; i++) fq_from_wire(r.c[i], p + i * fq_wb());
     f3_to_internal(r);
   }
   static __device__ __forceinline__ void to_wire(uint8_t* p, const El& a, bool zero) {
@@ -315,13 +370,14 @@ struct KF3 {                       // type d
     f3_to_reference(o);
     if (zero) f3_zero(o);
 #pragma unroll
-    for (int i = 0; i < 3; i++) fq_to_wire(p + i * kWS, o.c[i]);
+    for (int i = 0; i < 3; i++) fq_to_wire(p + i * fq_wb(), o.c[i]);
   }
 };
 
+#if !PBC_FQ_WIDE
 struct KF5 {                       // type g (19-byte coordinates)
   typedef F5 El;
-  static constexpr int kWire = 5 * kWG;
+  static __device__ __forceinline__ int wire() { return 5 * kWG; }
   static __device__ __forceinline__ void mul(El* r, const El* a, const El* b) { f5_mul(r, a, b); }
   static __device__ __forceinline__ void sqr(El* r, const El* a) { f5_sqr(r, a); }
   static __device__ __forceinline__ void inv(El* r, const El* a) { f5_inv(r, a); }
@@ -351,6 +407,8 @@ struct KF5 {                       // type g (19-byte coordinates)
   }
 };
 
+#endif
+
 // out[i] = k[i] * in[i] on the twist.  One thread per point; all temporaries that are passed by
 // address live at function scope (stack discipline note in pairing_f.cuh).
 template <class KF, int BLOCK>
@@ -360,8 +418,8 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
   El xP, yP, X, Y, Z, Z2, M, Y2, t, u, H, R;
-  KF::from_wire(xP, P + idx * (2 * KF::kWire));
-  KF::from_wire(yP, P + idx * (2 * KF::kWire) + KF::kWire);
+  KF::from_wire(xP, P + idx * (2 * KF::wire()));
+  KF::from_wire(yP, P + idx * (2 * KF::wire()) + KF::wire());
   // on the curve?  y^2 == (x^2 + a') x + b'
   KF::sqr(&t, &xP);
   KF::add_curve_a(t);
@@ -369,7 +427,7 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   KF::add_curve_b(t);
   KF::sqr(&u, &yP);
   bool ok = KF::eq(t, u);
-  uint32_t k[5];
+  uint32_t k[kZW];
   zr_from_wire(k, K + idx * c_zr.zlen);
   int top = zr_top_bit(k);
   X = xP;
@@ -430,10 +488,11 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   KF::mul(&X, &X, &u);
   KF::mul(&u, &u, &t);
   KF::mul(&Y, &Y, &u);
-  KF::to_wire(out + idx * (2 * KF::kWire), X, inf);
-  KF::to_wire(out + idx * (2 * KF::kWire) + KF::kWire, Y, inf);
+  KF::to_wire(out + idx * (2 * KF::wire()), X, inf);
+  KF::to_wire(out + idx * (2 * KF::wire()) + KF::wire(), Y, inf);
 }
 
+#if !PBC_FQ_WIDE
 // out[i] = in[i]^k[i] in GT (type f: 240-byte F_q^12 elements)
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
@@ -442,7 +501,7 @@ k_f_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
   F12 base, acc;
-  uint32_t k[5];
+  uint32_t k[kZW];
   f12_from_wire(base, G + idx * (12 * kWS));
   f12_to_internal(base);
   zr_from_wire(k, K + idx * c_zr.zlen);
@@ -457,6 +516,8 @@ k_f_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   f12_to_wire(out + idx * (12 * kWS), acc);
 }
 
+#endif
+
 // type d: 120-byte F_q^6 elements
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
@@ -465,8 +526,8 @@ k_d_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
   F6D base, acc;
-  uint32_t k[5];
-  f6d_from_wire(base, G + idx * (6 * kWS));
+  uint32_t k[kZW];
+  f6d_from_wire(base, G + idx * (6 * fq_wb()));
   f3_to_internal(base.a);
   f3_to_internal(base.b);
   zr_from_wire(k, K + idx * c_zr.zlen);
@@ -479,9 +540,10 @@ k_d_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   if (top < 0) f6d_one(acc);
   f3_to_reference(acc.a);
   f3_to_reference(acc.b);
-  f6d_to_wire(out + idx * (6 * kWS), acc);
+  f6d_to_wire(out + idx * (6 * fq_wb()), acc);
 }
 
+#if !PBC_FQ_WIDE
 // type g: 190-byte F_q^10 elements
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
@@ -490,7 +552,7 @@ k_g_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
   F10 base, acc;
-  uint32_t k[5];
+  uint32_t k[kZW];
   f10_from_wire(base, G + idx * (10 * kWG));
   zr_from_wire(k, K + idx * c_zr.zlen);
   int top = zr_top_bit(k);
@@ -502,5 +564,6 @@ k_g_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   if (top < 0) f10_one(acc);
   f10_to_wire(out + idx * (10 * kWG), acc);
 }
+#endif
 
 }  // namespace pbcb200

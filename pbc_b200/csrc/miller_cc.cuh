@@ -33,12 +33,14 @@
 
 namespace pbcb200 {
 
-struct CCConsts {
-  uint32_t A[kNS], B[kNS];     // curve y^2 = x^3 + A x + B over F_q (Montgomery form)
-  uint32_t r[kNS];             // group order (plain integer, little-endian words)
+template <int NS>
+struct CCConstsT {
+  uint32_t A[NS], B[NS];       // curve y^2 = x^3 + A x + B over F_q (Montgomery form)
+  uint32_t r[NS];              // group order (plain integer, little-endian words)
   uint32_t rbits;
   uint32_t a_is_zero;
 };
+typedef CCConstsT<kNS> CCConsts;
 __constant__ CCConsts c_cc;
 
 // PBC_CC_NAF = 1: the loop scans the non-adjacent form of r (host_naf.hpp) instead of its bits: one
@@ -228,7 +230,7 @@ __global__ void k_cc_pp_init(const uint8_t* __restrict__ P, uint32_t* __restrict
   if (blockIdx.x != 0 || threadIdx.x != 0) return;
   Fq xP, yP;
   fq_from_wire_w<WB>(xP, P);
-  fq_from_wire_w<WB>(yP, P + WB);
+  fq_from_wire_w<WB>(yP, P + wire_w<WB>());
   bool ok = cc_on_curve(xP, yP);
   TableSink sink{tab, 0};
   miller_cc_walk(sink, xP, yP);

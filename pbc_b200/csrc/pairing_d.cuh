@@ -16,17 +16,18 @@ namespace pbcb200 {
 struct F3 { Fq c[3]; };            // c0 + c1 x + c2 x^2
 struct F6D { F3 a, b; };           // a + b w,  w^2 = v
 
-struct DConsts {
-  uint32_t xpwr3[3][kNS];          // x^3 mod the field polynomial (arith/poly.c:1302-1333)
-  uint32_t xpwr4[3][kNS];          // x^4
-  uint32_t xpowq[3][kNS];          // x^q      (ecc/d_param.c:1043-1049)
-  uint32_t xpowq2[3][kNS];         // x^(2q)
-  uint32_t nqr[kNS];               // v
-  uint32_t nqrinv[kNS];            // 1/v    : untwisting factors (ecc/d_param.c:576-582)
-  uint32_t nqrinv2[kNS];           // 1/v^2
-  uint32_t twist_a[kNS];           // a v^2, b v^3: G2 curve over F_q^3 (ecc/curve.c:885-892)
-  uint32_t twist_b[kNS];
-  uint32_t two[kNS];               // Montgomery 2
+template <int NS>
+struct DConstsT {
+  uint32_t xpwr3[3][NS];          // x^3 mod the field polynomial (arith/poly.c:1302-1333)
+  uint32_t xpwr4[3][NS];          // x^4
+  uint32_t xpowq[3][NS];          // x^q      (ecc/d_param.c:1043-1049)
+  uint32_t xpowq2[3][NS];         // x^(2q)
+  uint32_t nqr[NS];               // v
+  uint32_t nqrinv[NS];            // 1/v    : untwisting factors (ecc/d_param.c:576-582)
+  uint32_t nqrinv2[NS];           // 1/v^2
+  uint32_t twist_a[NS];           // a v^2, b v^3: G2 curve over F_q^3 (ecc/curve.c:885-892)
+  uint32_t twist_b[NS];
+  uint32_t two[NS];               // Montgomery 2
   uint32_t phikonr[8];             // (q^2 - q + 1)/r, plain integer (ecc/d_param.c:1035-1041)
   uint32_t phibits;
   // Internal cubic basis (q = 2 mod 3; tools/proto_d_basis.py):  F_q^3 = F_q[w]/(w^3 + p w + 1) with
@@ -35,11 +36,12 @@ struct DConsts {
   // reference polynomial (xpwr3/xpwr4 rows).  xpowq / xpowq2 hold the values of the basis in use.
   uint32_t nice;
   uint32_t pad[2];
-  uint32_t pcoef[kNS];             // p
-  uint32_t bs[kNS], bs2[kNS], b2s[kNS];          // s, s^2, 2 s
-  uint32_t blam[kNS], blam2[kNS], blami[kNS], blami2[kNS];   // lam, lam^2, 1/lam, 1/lam^2
-  uint32_t qsqm[2][2 * kNS];       // q^2, 2 q^2 as plain double-width integers (offsets of the lazy F_q^3 product)
+  uint32_t pcoef[NS];             // p
+  uint32_t bs[NS], bs2[NS], b2s[NS];          // s, s^2, 2 s
+  uint32_t blam[NS], blam2[NS], blami[NS], blami2[NS];   // lam, lam^2, 1/lam, 1/lam^2
+  uint32_t qsqm[2][2 * NS];       // q^2, 2 q^2 as plain double-width integers (offsets of the lazy F_q^3 product)
 };
+typedef DConstsT<kNS> DConsts;
 __constant__ DConsts c_d;
 
 // ---------------------------------------------------------------------------------------------
@@ -378,18 +380,18 @@ k_d_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_
   } else {
     const uint8_t* p = P + idx * stride1;
     fq_from_wire(xP, p);
-    fq_from_wire(yP, p + kWS);
+    fq_from_wire(yP, p + fq_wb());
     ok = cc_on_curve(xP, yP);
   }
   DTower::Ctx ctx;
   F3 t, u;
   F6D v;
   Fq k;
-  const uint8_t* q = Q + idx * (6 * kWS);
+  const uint8_t* q = Q + idx * (6 * fq_wb());
 #pragma unroll
   for (int i = 0; i < 3; i++) {
-    fq_from_wire(ctx.Qx.c[i], q + i * kWS);
-    fq_from_wire(ctx.Qy.c[i], q + (3 + i) * kWS);
+    fq_from_wire(ctx.Qx.c[i], q + i * fq_wb());
+    fq_from_wire(ctx.Qy.c[i], q + (3 + i) * fq_wb());
   }
   f3_to_internal(ctx.Qx);
   f3_to_internal(ctx.Qy);
@@ -505,26 +507,26 @@ k_d_finalexp(const uint32_t* __restrict__ mv, const uint32_t* __restrict__ flag,
     f3_zero(out1);
     fq_one(out0.c[0]);
   }
-  uint8_t* o = out + idx * (6 * kWS);
+  uint8_t* o = out + idx * (6 * fq_wb());
 #pragma unroll 1
   for (int i = 0; i < 3; i++) {
-    fq_to_wire(o + i * kWS, out0.c[i]);
-    fq_to_wire(o + (3 + i) * kWS, out1.c[i]);
+    fq_to_wire(o + i * fq_wb(), out0.c[i]);
+    fq_to_wire(o + (3 + i) * fq_wb(), out1.c[i]);
   }
 }
 
 __device__ __forceinline__ void f6d_from_wire(F6D& v, const uint8_t* p) {
 #pragma unroll 1
   for (int i = 0; i < 3; i++) {
-    fq_from_wire(v.a.c[i], p + i * kWS);
-    fq_from_wire(v.b.c[i], p + (3 + i) * kWS);
+    fq_from_wire(v.a.c[i], p + i * fq_wb());
+    fq_from_wire(v.b.c[i], p + (3 + i) * fq_wb());
   }
 }
 __device__ __forceinline__ void f6d_to_wire(uint8_t* p, const F6D& v) {
 #pragma unroll 1
   for (int i = 0; i < 3; i++) {
-    fq_to_wire(p + i * kWS, v.a.c[i]);
-    fq_to_wire(p + (3 + i) * kWS, v.b.c[i]);
+    fq_to_wire(p + i * fq_wb(), v.a.c[i]);
+    fq_to_wire(p + (3 + i) * fq_wb(), v.b.c[i]);
   }
 }
 
@@ -535,8 +537,8 @@ __global__ void k_d_tower_op(int op, uint8_t* __restrict__ out, const uint8_t* _
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n) return;
   F6D x, y, r;
-  f6d_from_wire(x, a + idx * (6 * kWS));
-  f6d_from_wire(y, b + idx * (6 * kWS));
+  f6d_from_wire(x, a + idx * (6 * fq_wb()));
+  f6d_from_wire(y, b + idx * (6 * fq_wb()));
   f3_to_internal(x.a); f3_to_internal(x.b); f3_to_internal(y.a); f3_to_internal(y.b);
   switch (op) {
     case 0: f6d_mul(&r, &x, &y); break;
@@ -547,7 +549,7 @@ __global__ void k_d_tower_op(int op, uint8_t* __restrict__ out, const uint8_t* _
     default: f3_inv(&r.a, &x.a); f3_zero(r.b); break;
   }
   f3_to_reference(r.a); f3_to_reference(r.b);
-  f6d_to_wire(out + idx * (6 * kWS), r);
+  f6d_to_wire(out + idx * (6 * fq_wb()), r);
 }
 
 }  // namespace pbcb200

@@ -28,9 +28,11 @@
 #include "pairing_f.cuh"
 #include "pairing_f_slots.cuh"
 #include "pairing_g.cuh"
+#include "pairing_e.cuh"
 #include "group_a.cuh"
 #include "group_a1.cuh"
 #include "group_cc.cuh"
+#include "group_e.cuh"
 #include "engine_d_wide.h"
 
 #if defined(PBC_HOST_SIM) && !defined(PBC_HOST_SIM_D_WIDE)
@@ -141,7 +143,7 @@ struct DevCtx {
 };
 
 struct pbc_b200_pairing_s {
-  int type = 0;                // 'a', 'f', 'd', 'g'; '1' = a1
+  int type = 0;                // 'a', 'e', 'f', 'd', 'g'; '1' = a1
   int g1_len = 0, g2_len = 0, gt_len = 0;
   int nlimbs = 0;
   bool full = false;
@@ -153,6 +155,8 @@ struct pbc_b200_pairing_s {
   A1Naf a1naf;
 #endif
   size_t a1_rows = 0;          // rows of the fixed-argument line table (3 per tangent / chord)
+  EConsts e;                   // type e (also uses fp, a1.wb and a1g.n / zlen: the 34-limb pieces of type a1)
+  uint32_t e_pts[4 * kNA1];    // a, b, x(R), y(R), Montgomery form (g_e_pts)
   size_t cc_rows = 0;          // types f, d, g: lines of the Miller walk (computed once at init)
   CCConsts cc;
 #if PBC_CC_NAF
@@ -218,6 +222,8 @@ struct Job {
 };
 
 static size_t cc_table_bytes(const pbc_b200_pairing_s* p);
+// type e: the fixed-argument table (pairing_e.cuh, e_pp_rows) and its flag word
+static size_t e_table_bytes(const pbc_b200_pairing_s* p) { return (e_pp_rows(p->e.exp2) * kNA1 + 4) * 4; }
 
 // workspace bytes for n_out outputs of `job`
 static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out) {
@@ -227,6 +233,14 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
     if (job.mode == kSingle) return n_out * (2 + 1 + 1 + 2) * fq;
     if (job.mode == kProd) return n_out * job.k * (2 + 1 + 2) * fq + n_out * (2 + 1 + 1) * fq;
     return n_out * (2 + 1 + 1) * fq + (p->a1_rows * kNA1 + 4) * 4;
+  }
+  if (p->type == 'e') {
+    // f, dprod, prefix per output; Miller inputs add f, d, x(P), Q + R [5] and the save [5]; pp adds
+    // the save [2] and (one-shot) the line table
+    const size_t fq = (size_t)kNA1 * 4;
+    if (job.mode == kSingle) return n_out * (3 + kQWords + kSWords) * fq;
+    if (job.mode == kProd) return n_out * job.k * (3 + kQWords + kSWords) * fq + n_out * 3 * fq;
+    return n_out * (3 + 2) * fq + e_table_bytes(p);
   }
   if (p->type == 'a') {
     const size_t fq = 64;
@@ -853,6 +867,156 @@ static int init_type_g(pbc_b200_pairing_s* p, const std::map<std::string, std::s
   return 0;
 }
 
+// a square root of t mod q (Tonelli-Shanks; t a square), host side.  Returns 0 where no root is found
+// (every loop is bounded: q comes from the caller's parameter text and need not be prime).
+static BigUInt host_sqrt(const BigUInt& t, const BigUInt& q) {
+  const BigUInt one(1), two(2), qm1 = q - one;
+  BigUInt Q = qm1, z(2);
+  uint32_t s = 0;
+  while (!Q.bit(0)) { Q = Q / two; s++; }
+  for (int tries = 0; !(BigUInt::powmod(z, qm1 / two, q) == qm1); tries++) {
+    if (tries == 200) return BigUInt();
+    z = z + one;
+  }
+  BigUInt c = BigUInt::powmod(z, Q, q), x = BigUInt::powmod(t, (Q + one) / two, q), b = BigUInt::powmod(t, Q, q);
+  uint32_t m = s;
+  while (!(b == one) && !b.is_zero()) {
+    uint32_t i = 0;
+    BigUInt b2 = b;
+    while (!(b2 == one) && i < m) { b2 = BigUInt::mulmod(b2, b2, q); i++; }
+    if (i == m) return BigUInt();
+    BigUInt g = c;
+    for (uint32_t j = 0; j + 1 < m - i; j++) g = BigUInt::mulmod(g, g, q);
+    x = BigUInt::mulmod(x, g, q);
+    c = BigUInt::mulmod(g, g, q);
+    b = BigUInt::mulmod(b, c, q);
+    m = i;
+  }
+  return b.is_zero() ? BigUInt() : x;
+}
+
+// k P == O on y^2 = x^3 + a x + b over F_q, P affine (host side, Jacobian: no inversions)
+static bool host_mul_is_inf(const BigUInt& k, const BigUInt& px, const BigUInt& py, const BigUInt& a, const BigUInt& q) {
+  BigUInt X, Y, Z;                                 // Z = 0: O
+  auto mm = [&](const BigUInt& u, const BigUInt& v) { return BigUInt::mulmod(u, v, q); };
+  auto ad = [&](const BigUInt& u, const BigUInt& v) { return BigUInt::addmod(u, v, q); };
+  auto sb = [&](const BigUInt& u, const BigUInt& v) { return BigUInt::submod(u, v, q); };
+  auto dbl = [&]() {
+    if (Z.is_zero() || Y.is_zero()) { Z = BigUInt(); return; }
+    BigUInt Z2 = mm(Z, Z), X2 = mm(X, X), Y2 = mm(Y, Y);
+    BigUInt M = ad(ad(ad(X2, X2), X2), mm(a, mm(Z2, Z2)));
+    BigUInt S = mm(X, Y2);
+    S = ad(S, S); S = ad(S, S);
+    BigUInt Y4 = mm(Y2, Y2), E8 = ad(Y4, Y4);
+    E8 = ad(E8, E8); E8 = ad(E8, E8);
+    BigUInt Xn = sb(sb(mm(M, M), S), S);
+    Z = mm(Y, Z); Z = ad(Z, Z);
+    Y = sb(mm(M, sb(S, Xn)), E8);
+    X = Xn;
+  };
+  for (size_t i = k.bits(); i-- > 0;) {
+    dbl();
+    if (!k.bit(i)) continue;
+    if (Z.is_zero()) { X = px; Y = py; Z = BigUInt(1); continue; }
+    BigUInt Z2 = mm(Z, Z), H = sb(mm(px, Z2), X), R = sb(mm(py, mm(Z2, Z)), Y);
+    if (H.is_zero()) {
+      if (R.is_zero()) dbl(); else Z = BigUInt();
+      continue;
+    }
+    BigUInt H2 = mm(H, H), H3 = mm(H2, H), U = mm(X, H2);
+    BigUInt Xn = sb(sb(sb(mm(R, R), H3), U), U);
+    Y = sb(mm(R, sb(U, Xn)), mm(Y, H3));
+    Z = mm(Z, H);
+    X = Xn;
+  }
+  return Z.is_zero();
+}
+
+// e_init_pairing (ecc/e_param.c:840-880), k = 1.  34-limb field (type a1's slot machine): q below 2^1087.
+static int init_type_e(pbc_b200_pairing_s* p, const std::map<std::string, std::string>& tab) {
+  BigUInt q, r, h, a, b;
+  int exp2, exp1, sign1, sign0;
+  if (!get_big(tab, "q", &q) || !get_big(tab, "r", &r) || !get_big(tab, "h", &h) || !get_big(tab, "a", &a) ||
+      !get_big(tab, "b", &b)) return 1;
+  if (!get_int(tab, "exp2", &exp2) || !get_int(tab, "exp1", &exp1) ||
+      !get_int(tab, "sign1", &sign1) || !get_int(tab, "sign0", &sign0)) return 1;
+  if (q.bits() > 32 * (size_t)kNA1 - 1) return fail("type e: this build supports q below 2^%d (got %zu bits)", 32 * kNA1 - 1, q.bits());
+  if (q.bits() < 64) return fail("type e: q too small");
+  if ((sign1 != 1 && sign1 != -1) || (sign0 != 1 && sign0 != -1)) return fail("type e: sign1 and sign0 must be 1 or -1");
+  if (exp1 <= 0 || exp2 <= exp1 || exp2 >= 32 * kNA1 - 1) return fail("type e: bad exp1/exp2");
+  const BigUInt one(1), p2 = one.shl((size_t)exp2), p1 = one.shl((size_t)exp1);
+  BigUInt rr = sign1 > 0 ? p2 + p1 : p2 - p1;
+  rr = sign0 > 0 ? rr + one : rr - one;
+  if (!(rr == r)) return fail("type e: r != 2^exp2 + sign1 2^exp1 + sign0");
+  BigUInt ph, rem;
+  BigUInt::divmod(q - one, r, &ph, &rem);
+  if (!rem.is_zero()) return fail("type e: r does not divide q - 1");
+  a = a % q;
+  b = b % q;
+  p->type = 'e';
+  memset(&p->zr, 0, sizeof p->zr);
+  p->zr.zlen = (uint32_t)((r.bits() + 7) / 8);
+  p->zr_len = (int)p->zr.zlen;
+  p->nlimbs = kNA1;
+  p->full = false;
+  const int wb = (int)((q.bits() + 7) / 8);
+  p->g1_len = p->g2_len = 2 * wb;
+  p->gt_len = wb;
+  fill_fp_consts(&p->fp, q, kNA1);
+  memset(&p->a1, 0, sizeof p->a1);
+  p->a1.wb = (uint32_t)wb;
+  memset(&p->a1g, 0, sizeof p->a1g);
+  r.to_words(p->a1g.n, kNA1);                      // scalars are reduced mod r (a1_zr_from_wire)
+  p->a1g.zlen = p->zr.zlen;
+  p->a1g.count = (uint32_t)wb;
+  p->hash_ok = false;                              // element_from_hash / compressed points: not for type e
+  // R: the first x = 1, 2, .. with x^3 + a x + b a non-zero square, y the smaller root, r R != O
+  BigUInt Rx, Ry;
+  bool found = false;
+  for (uint64_t x = 1; !found && x < 1000; x++) {
+    BigUInt X(x), t = BigUInt::addmod(BigUInt::mulmod(BigUInt::addmod(BigUInt::mulmod(X, X, q), a, q), X, q), b, q);
+    if (t.is_zero() || !(BigUInt::powmod(t, (q - one) / BigUInt(2), q) == one)) continue;
+    BigUInt y = host_sqrt(t, q);
+    if (!(BigUInt::mulmod(y, y, q) == t)) continue;
+    if (q - y < y) y = q - y;
+    if (host_mul_is_inf(r, X, y, a, q)) continue;
+    Rx = X;
+    Ry = y;
+    found = true;
+  }
+  if (!found) return fail("type e: found no point R outside E[r]");
+  p->derived["R"] = {Rx, Ry};
+  p->derived["phikonr"] = {ph};
+  memset(p->e_pts, 0, sizeof p->e_pts);
+  to_mont(p->e_pts + kEA * kNA1, a, q, kNA1);
+  to_mont(p->e_pts + kEB * kNA1, b, q, kNA1);
+  to_mont(p->e_pts + kERX * kNA1, Rx, q, kNA1);
+  to_mont(p->e_pts + kERY * kNA1, Ry, q, kNA1);
+  EConsts& c = p->e;
+  memset(&c, 0, sizeof c);
+  c.exp1 = (uint32_t)exp1;
+  c.exp2 = (uint32_t)exp2;
+  c.sign1 = sign1;
+  c.sign0 = sign0;
+  c.a_zero = a.is_zero() ? 1u : 0u;
+  // final exponent (q - 1)/r as a left-to-right window of width 4: scanning down from the top bit,
+  // each window starts at a set bit and ends at the lowest set bit of the 4 below it
+  if (ph.bits() > sizeof c.dig) return fail("type e: final exponent too large");
+  int i = (int)ph.bits() - 1;
+  bool first = true;
+  while (i >= 0) {
+    if (!ph.bit((size_t)i)) { i--; continue; }
+    int j = i - 3 < 0 ? 0 : i - 3;
+    while (!ph.bit((size_t)j)) j++;
+    uint32_t d = 0;
+    for (int k = i; k >= j; k--) d = 2 * d + (ph.bit((size_t)k) ? 1u : 0u);
+    c.dig[j] = (uint8_t)d;
+    if (first) { c.dstart = (uint32_t)j; first = false; }
+    i = j - 1;
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 // device contexts
 // ------------------------------------------------------------------------------------------
@@ -903,6 +1067,14 @@ static constexpr size_t kSmemInv34 = (size_t)5 * kSlotA1 * kBlockA1Small;
 // so the code generated for the measured pairing kernels does not move when these change
 static constexpr int kBlockA1G = 64;
 static constexpr size_t kSmemA1G = (size_t)kGSlots * kSlotA1 * kBlockA1G;   // 11 slots: 93.5 KB, two blocks per SM
+// type e: the same 34-limb slots; Miller kernel 13 slots * 136 B * 128 threads = 221 KB, one block per SM
+static constexpr int kBlockE = 128;
+static constexpr size_t kSmemEMiller = (size_t)kESlots * kSlotA1 * kBlockE;
+static constexpr size_t kSmemEFinal = (size_t)kEFinalSlots * kSlotA1 * kBlockA1Small;
+static constexpr size_t kSmemEProd = (size_t)kEProdSlots * kSlotA1 * kBlockA1Small;
+static constexpr size_t kSmemEPP = (size_t)kEPPSlots * kSlotA1 * kBlockA1Small;
+static constexpr size_t kSmemEPPInit = (size_t)kEPPInitSlots * kSlotA1 * 32;
+static constexpr size_t kSmemEGroup = (size_t)kEGroupSlots * kSlotA1 * kBlockA1G;
 
 static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
   if ((int)p->ctx.size() <= dev) p->ctx.resize(dev + 1);
@@ -945,6 +1117,19 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
       CUDA_OK(allow_smem(k_a1_gt_mul<kBlockA1G>, (size_t)7 * kSlotA1 * kBlockA1G));
       CUDA_OK(allow_smem(k_a1_g1_decompress<kBlockA1G>, (size_t)5 * kSlotA1 * kBlockA1G));
     }
+    if (p->type == 'e') {
+      CUDA_OK(allow_smem(k_e_miller<kBlockE>, kSmemEMiller));
+      CUDA_OK(allow_smem(k_e_prod<kBlockA1Small>, kSmemEProd));
+      CUDA_OK(allow_smem(k_e_pp_init<32>, kSmemEPPInit));
+      CUDA_OK(allow_smem(k_e_pp_apply<kBlockA1Small>, kSmemEPP));
+      CUDA_OK(allow_smem(k_e_finalexp<kBlockA1Small>, kSmemEFinal));
+      CUDA_OK(allow_smem(k_batch_invert<kNA1, false, kBlockA1Small>, kSmemInv34));
+      CUDA_OK(allow_smem(k_a1_fp_op<kBlockA1Small>, (size_t)4 * kSlotA1 * kBlockA1Small));
+      CUDA_OK(allow_smem(k_e_g1_mul<kBlockA1G>, kSmemA1G));
+      CUDA_OK(allow_smem(k_a1_g1_finish<kBlockA1G>, (size_t)4 * kSlotA1 * kBlockA1G));
+      CUDA_OK(allow_smem(k_e_gt_pow<kBlockA1G>, kSmemEGroup));
+      CUDA_OK(allow_smem(k_e_gt_mul<kBlockA1G>, kSmemEGroup));
+    }
     c.ready = true;
   }
   // make this handle's constants resident on the device
@@ -974,6 +1159,12 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
     if (p->type == 'a') CUDA_OK(cudaMemcpyToSymbol(c_a, &p->a, sizeof(AConsts)));
     if (p->type == '1') CUDA_OK(cudaMemcpyToSymbol(c_a1, &p->a1, sizeof(A1Consts)));
     if (p->type == '1') CUDA_OK(cudaMemcpyToSymbol(c_a1g, &p->a1g, sizeof(A1GroupConsts)));
+    if (p->type == 'e') {                  // type a1's wire width and scalar order, and the type e block
+      CUDA_OK(cudaMemcpyToSymbol(c_a1, &p->a1, sizeof(A1Consts)));
+      CUDA_OK(cudaMemcpyToSymbol(c_a1g, &p->a1g, sizeof(A1GroupConsts)));
+      CUDA_OK(cudaMemcpyToSymbol(c_e, &p->e, sizeof(EConsts)));
+      CUDA_OK(cudaMemcpyToSymbol(g_e_pts, p->e_pts, sizeof p->e_pts));
+    }
 #if PBC_A1_NAF
     if (p->type == '1') CUDA_OK(cudaMemcpyToSymbol(c_a1naf, &p->a1naf, sizeof(A1Naf)));
 #endif
@@ -1097,6 +1288,59 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     STAGE(2);
     unsigned gf = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
     k_a1_finalexp<kBlockA1Small><<<gf, kBlockA1Small, kSmemA1Final, st>>>(f, dprod, d_out, n);
+    LAUNCHED();
+    STAGE(3);
+    CUDA_OK(cudaGetLastError());
+    return 0;
+  }
+  if (p->type == 'e') {
+    // limb-major arrays of 34-limb elements: E = 17 uint2 vectors per element
+    const size_t E = kNA1 / 2;
+    uint2 *f, *dprod, *prefix;
+    const size_t wire = (size_t)p->g1_len;
+    STAGE(0);
+    if (job.mode == kSingle || job.mode == kProd) {
+      const size_t m = job.mode == kProd ? n * job.k : n;
+      uint2* fi = (uint2*)ws;                    // [E][m]
+      uint2* di = fi + E * m;                    // [E][m]
+      uint2* px = di + E * m;                    // [E][m]
+      uint2* qd = px + E * m;                    // [kQWords][E][m]
+      uint2* sv = qd + kQWords * E * m;          // [kSWords][E][m]
+      unsigned gm = (unsigned)((m + kBlockE - 1) / kBlockE);
+      k_e_miller<kBlockE><<<gm, kBlockE, kSmemEMiller, st>>>(d_in1, d_in2, fi, di, px, qd, sv, m, wire);
+      LAUNCHED();
+      if (job.mode == kSingle) {
+        f = fi;
+        dprod = di;
+        prefix = px;                             // x(P) is dead once the Miller kernel has finished
+      } else {
+        f = sv + kSWords * E * m;                // [E][n]
+        dprod = f + E * n;
+        prefix = dprod + E * n;
+        unsigned gp = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
+        k_e_prod<kBlockA1Small><<<gp, kBlockA1Small, kSmemEProd, st>>>(fi, di, f, dprod, job.k, n, m);
+        LAUNCHED();
+      }
+    } else {
+      f = (uint2*)ws;
+      dprod = f + E * n;
+      prefix = dprod + E * n;
+      uint2* pv = prefix + E * n;                // [2][E][n]
+      uint32_t* tab = (uint32_t*)(pv + 2 * E * n);
+      if (job.pp_tab) tab = (uint32_t*)job.pp_tab;
+      else { k_e_pp_init<32><<<1, 32, kSmemEPPInit, st>>>(d_in1, tab); LAUNCHED(); }
+      unsigned gm = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
+      k_e_pp_apply<kBlockA1Small><<<gm, kBlockA1Small, kSmemEPP, st>>>(tab, d_in2, f, dprod, pv, n);
+      LAUNCHED();
+    }
+    STAGE(1);
+    size_t T = inv_threads(p, n, 128);
+    unsigned gi = (unsigned)((T + kBlockA1Small - 1) / kBlockA1Small);
+    k_batch_invert<kNA1, false, kBlockA1Small><<<gi, kBlockA1Small, kSmemInv34, st>>>(dprod, prefix, n, T);
+    LAUNCHED();
+    STAGE(2);
+    unsigned gf = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
+    k_e_finalexp<kBlockA1Small><<<gf, kBlockA1Small, kSmemEFinal, st>>>(f, dprod, d_out, n);
     LAUNCHED();
     STAGE(3);
     CUDA_OK(cudaGetLastError());
@@ -1359,7 +1603,8 @@ int pbc_b200_pairing_init_set_buf(pbc_b200_pairing_t** out, const char* param, s
   else if (it->second == "f") rc = init_type_f(p, tab);
   else if (it->second == "d") rc = init_type_d(p, tab);
   else if (it->second == "g") rc = init_type_g(p, tab);
-  else rc = fail("pairing type `%s' is not on the GPU hot path (supported: a, a1, d with k = 6, f, g)", it->second.c_str());
+  else if (it->second == "e") rc = init_type_e(p, tab);
+  else rc = fail("pairing type `%s' is not on the GPU hot path (supported: a, a1, d with k = 6, e, f, g)", it->second.c_str());
   if (rc) { delete p; return 1; }
   if (p->type == 'f' || p->type == 'd' || p->type == 'g') p->cc_rows = cc_table_rows_compute(p);
   *out = p;
@@ -1451,7 +1696,7 @@ struct pbc_b200_pp_s {
   pbc_b200_pairing_s* p = nullptr;
   int dev = 0;
   uint8_t* d_in1 = nullptr;     // wire bytes of the fixed first argument
-  void* d_tab = nullptr;        // types a, a1: line-coefficient table
+  void* d_tab = nullptr;        // line-coefficient table
 };
 
 int pbc_b200_pp_init(pbc_b200_pairing_t* p, pbc_b200_pp_t** out, const unsigned char* in1) {
@@ -1470,6 +1715,7 @@ int pbc_b200_pp_init(pbc_b200_pairing_t* p, pbc_b200_pp_t** out, const unsigned 
   size_t tab_bytes = 0;
   if (p->type == 'a') tab_bytes = (size_t)(3 * (p->a.exp2 + 1) * kNA + 4) * 4;
   if (p->type == '1') tab_bytes = (p->a1_rows * kNA1 + 4) * 4;
+  if (p->type == 'e') tab_bytes = e_table_bytes(p);
   const bool cc = p->type == 'f' || p->type == 'd' || p->type == 'g';
   if (cc) tab_bytes = cc_table_bytes(p);
   cudaError_t e = cudaMalloc(&pp->d_in1, (size_t)p->g1_len);
@@ -1477,6 +1723,7 @@ int pbc_b200_pp_init(pbc_b200_pairing_t* p, pbc_b200_pp_t** out, const unsigned 
   if (e == cudaSuccess) e = cudaMemcpyAsync(pp->d_in1, in1, (size_t)p->g1_len, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess && p->type == 'a') { k_a_pp_init<32><<<1, 32, kSmemAPPInit, st>>>(pp->d_in1, (uint32_t*)pp->d_tab); LAUNCHED(); }
   if (e == cudaSuccess && p->type == '1') { k_a1_pp_init<32><<<1, 32, kSmemA1PPInit, st>>>(pp->d_in1, (uint32_t*)pp->d_tab, p->a1_rows); LAUNCHED(); }
+  if (e == cudaSuccess && p->type == 'e') { k_e_pp_init<32><<<1, 32, kSmemEPPInit, st>>>(pp->d_in1, (uint32_t*)pp->d_tab); LAUNCHED(); }
   if (e == cudaSuccess && cc) {
     if (p->dwide) pbcb200_dw::dw_pp_init(pp->d_in1, (uint32_t*)pp->d_tab, cc_table_rows(p), st);
     else if (p->type == 'g') k_cc_pp_init<kWG><<<1, 32, 0, st>>>(pp->d_in1, (uint32_t*)pp->d_tab, cc_table_rows(p));
@@ -1563,7 +1810,7 @@ void pbc_b200_host_free(void* ptr) { if (ptr) cudaFreeHost(ptr); }
 // smem > 0 (type a, the slot multiplier of mode 1 only): launch with that much dynamic shared memory per block
 static double bench_fpmul(pbc_b200_pairing_t* p, int mode, int blocks, int iters, int reps, size_t smem) {
   if (!p) { fail("null argument"); return -1; }
-  if (p->type == '1') { fail("bench_fpmul: not built for type a1"); return -1; }
+  if (p->type == '1' || p->type == 'e') { fail("bench_fpmul: not built for the 34-limb field (types a1, e)"); return -1; }
   if (p->dwide) { fail("bench_fpmul: not built for the eight-limb type d field"); return -1; }
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || ctx_prepare(p, dev)) return -1;
@@ -1696,6 +1943,28 @@ static int enqueue_group(pbc_b200_pairing_s* p, int which /*0 = G1, 1 = GT, 2 = 
     CUDA_OK(cudaGetLastError());
     return 0;
   }
+  if (p->type == 'e') {
+    unsigned g = (unsigned)((n + kBlockA1G - 1) / kBlockA1G);
+    if (which == 0 || which == 2) {                // type e: G2 = G1 (ecc/e_param.c:874)
+      const size_t E = kNA1 / 2;
+      uint2* xyz = (uint2*)ws;                  // [2][E][n]  (X, Y)
+      uint2* zarr = xyz + 2 * E * n;            // [E][n]
+      uint2* prefix = zarr + E * n;             // [E][n]
+      k_e_g1_mul<kBlockA1G><<<g, kBlockA1G, kSmemA1G, st>>>(d_in, d_k, xyz, zarr, n);
+      LAUNCHED();
+      size_t T = inv_threads(p, n, 128);
+      unsigned gi = (unsigned)((T + kBlockA1Small - 1) / kBlockA1Small);
+      k_batch_invert<kNA1, false, kBlockA1Small><<<gi, kBlockA1Small, kSmemInv34, st>>>(zarr, prefix, n, T);
+      LAUNCHED();
+      k_a1_g1_finish<kBlockA1G><<<g, kBlockA1G, (size_t)4 * kSlotA1 * kBlockA1G, st>>>(xyz, zarr, d_out, n);
+      LAUNCHED();
+    } else {
+      k_e_gt_pow<kBlockA1G><<<g, kBlockA1G, kSmemEGroup, st>>>(d_in, d_k, d_out, n);
+      LAUNCHED();
+    }
+    CUDA_OK(cudaGetLastError());
+    return 0;
+  }
   if (p->type == 'a') {
     if (which == 0 || which == 2) {                // type a: G2 = G1 (ecc/a_param.c:1461-1462)
       uint4* xyz = (uint4*)ws;                 // [2][4][n]  (X, Y)
@@ -1747,7 +2016,7 @@ static int run_group(pbc_b200_pairing_s* p, int which, unsigned char* out, const
   DevCtx& c = p->ctx[dev];
   size_t elen = which == 0 ? (size_t)p->g1_len : (which == 2 ? (size_t)p->g2_len : (size_t)p->gt_len);
   size_t wsb = p->type == 'a' && which != 1 ? n * 64 * (2 + 1 + 1) : 16;
-  if (p->type == '1' && which != 1) wsb = n * kSlotA1 * (2 + 1 + 1);
+  if ((p->type == '1' || p->type == 'e') && which != 1) wsb = n * kSlotA1 * (2 + 1 + 1);
   size_t stage = device ? 0 : n * (2 * elen + (size_t)p->zr_len);
   if (c.cap_dev < wsb + stage) {
     CUDA_OK(cudaDeviceSynchronize());
@@ -1807,6 +2076,7 @@ int pbc_b200_gt_pow_zn_device(pbc_b200_pairing_t* p, void* d_out, const void* d_
 static int run_from_hash(pbc_b200_pairing_s* p, unsigned char* out, const unsigned char* data, size_t len, size_t n,
                          bool device, void* stream) {
   if (!p || (n && (!out || !data))) return fail("null argument");
+  if (p->type == 'e') return fail("element_from_hash: not available for type e (q = 1 mod 16 needs a 34-limb Tonelli-Shanks)");
   if (p->type != '1' && !p->hash_ok) return fail("element_from_hash: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q) and a cofactor below 2^384");
   if (len == 0 || len > (1u << 20)) return fail("element_from_hash: hash length must be 1..2^20 bytes");
   if (n == 0) return 0;
@@ -1893,6 +2163,7 @@ extern "C" int pbc_b200_pairing_length_in_bytes_compressed_G1(const pbc_b200_pai
 extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in,
                                                  size_t n) {
   if (!p || (n && (!out || !in))) return fail("null argument");
+  if (p->type == 'e') return fail("element_from_bytes_compressed: not available for type e");
   if (p->type != '1' && !p->hash_ok) return fail("element_from_bytes_compressed: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q)");
   if (n == 0) return 0;
   std::lock_guard<std::mutex> lk(p->mu);
@@ -1946,6 +2217,9 @@ static int enqueue_gt_mul(pbc_b200_pairing_s* p, uint8_t* d_out, const uint8_t* 
   if (p->type == 'a') {
     unsigned g = (unsigned)((n + kBlockMiller - 1) / kBlockMiller);
     k_a_gt_mul<kBlockMiller><<<g, kBlockMiller, (size_t)7 * 64 * kBlockMiller, st>>>(d_a, d_b, d_out, n);
+  } else if (p->type == 'e') {
+    unsigned g = (unsigned)((n + kBlockA1G - 1) / kBlockA1G);
+    k_e_gt_mul<kBlockA1G><<<g, kBlockA1G, kSmemEGroup, st>>>(d_a, d_b, d_out, n);
   } else if (p->type == '1') {
     unsigned g = (unsigned)((n + kBlockA1G - 1) / kBlockA1G);
     k_a1_gt_mul<kBlockA1G><<<g, kBlockA1G, (size_t)7 * kSlotA1 * kBlockA1G, st>>>(d_a, d_b, d_out, n);
@@ -2145,7 +2419,7 @@ extern "C" int pbc_b200_fp_op(pbc_b200_pairing_t* p, int op, unsigned char* out,
   CUDA_OK(cudaMemcpy(da.p, a, n * wb, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(db.p, b ? b : a, n * wb, cudaMemcpyHostToDevice));
   unsigned g = (unsigned)((n + 127) / 128);
-  if (p->type == '1') {
+  if (p->type == '1' || p->type == 'e') {
     k_a1_fp_op<kBlockA1Small><<<g, kBlockA1Small, (size_t)4 * kSlotA1 * kBlockA1Small>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
   } else if (p->type == 'a') {
     CUDA_OK(allow_smem(k_fp_op<kNA, true, 64, 128>, 4 * 64 * 128));

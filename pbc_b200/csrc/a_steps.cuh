@@ -33,88 +33,9 @@ PBC_STEP void a_fmul(int f0, int f1, int l0, int l1, int t0, int t1, int t2) {
 
 // One Miller doubling step:  f <- f^2 * l_{V,V}(phi(Q)),  V <- 2V   (Jacobian, a = 1).
 // 13 multiplications + 6 squarings (reference: 23 multiplications, ecc/a_param.c:1082-1139).
-template <class O>
-PBC_STEP void a_double_step() {
-  // f = f^2  (arith/fieldquadratic.c:459-477)
-  O::add(aT0, aF0, aF1);
-  O::sub(aT1, aF0, aF1);
-  O::mul(aF1, aF0, aF1);
-  O::dbl(aF1, aF1);
-  O::mul(aF0, aT0, aT1);
-  // M = 3 X^2 + Z^4
-  O::sqr(aT0, aX);
-  O::sqr(aT1, aZ2);
-  O::dbl(aT2, aT0);
-  O::add(aT0, aT0, aT2);
-  O::add(aT0, aT0, aT1);
-  O::sqr(aT1, aY);                 // Y^2
-  O::mul(aT2, aX, aT1);
-  O::dbl(aT2, aT2, 2);             // S = 4 X Y^2
-  O::mul(aT3, aT0, aZ2);           // M Z^2
-  O::mul(aT4, aT3, aQX);
-  O::mul(aT5, aX, aT0);
-  O::sub(aT5, aT5, aT1);
-  O::sub(aT5, aT5, aT1);
-  O::add(aT4, aT4, aT5);           // Re l = X M - 2 Y^2 + M Z^2 Qx
-  O::mul(aZ, aY, aZ);
-  O::dbl(aZ, aZ);                  // Z' = 2 Y Z
-  O::mul(aT3, aZ, aZ2);
-  O::mul(aT3, aT3, aQY);           // Im l = Z' Z^2 Qy
-  O::sqr(aZ2, aZ);
-  O::sqr(aT5, aT0);
-  O::sub(aX, aT5, aT2);
-  O::sub(aX, aX, aT2);             // X' = M^2 - 2 S
-  O::sqr(aT1, aT1);
-  O::dbl(aT1, aT1, 3);             // 8 Y^4
-  O::sub(aT2, aT2, aX);
-  O::mul(aY, aT0, aT2);
-  O::sub(aY, aY, aT1);             // Y' = M (S - X') - 8 Y^4
-  a_fmul<O>(aF0, aF1, aT4, aT3, aT0, aT1, aT2);
-}
-
-// Chord through V = (X, Y, Z) (Jacobian, Z2 = Z^2) and the affine point P = (xP, yP) held in
-// slots sPX, sPY (clobbered), evaluated at phi(Q); then V <- V + P.
-// Device replacement for compute_abc_line_proj + a_miller_evalfn + proj_add of a1_pairing_proj
-// (ecc/a_param.c:1820-1837, :306-315, :1869-1896); same line, same point, fewer products:
-//   H = xP Z^2 - X,  R = yP Z^3 - Y
-//   a = -R,  b = H Z (= Z of the sum),  c = yP Z X - xP Y;   l(phi(Q)) = (c - a Qx) + i (b Qy)
-//   X3 = R^2 - H^3 - 2 X H^2,  Y3 = R (X H^2 - X3) - Y H^3,  Z3 = b
-// 16 multiplications + 3 squarings including the f update.  Temporaries: aT0..aT3 and aZ2.
-template <class O>
-PBC_STEP void a1_chord_add(int sPX, int sPY) {
-  O::mul(aT0, aZ2, aZ);            // Z^3
-  O::mul(aT1, sPX, aZ2);
-  O::sub(aT1, aT1, aX);            // H
-  O::mul(aT0, sPY, aT0);           // yP Z^3
-  O::sub(aT2, aY, aT0);            // a = Y - yP Z^3
-  O::sub(aT0, aT0, aY);            // R
-  O::mul(aT3, sPY, aZ);
-  O::mul(aT3, aT3, aX);            // yP Z X
-  O::mul(sPX, sPX, aY);            // xP Y
-  O::sub(aT3, aT3, sPX);           // c
-  O::mul(aZ, aT1, aZ);             // b = H Z
-  O::mul(aT2, aT2, aQX);
-  O::sub(aT2, aT3, aT2);           // Re l = c - a Qx
-  O::mul(sPX, aZ, aQY);            // Im l = b Qy
-  a_fmul<O>(aF0, aF1, aT2, sPX, aT3, sPY, aZ2);
-  O::sqr(aT2, aT1);                // H^2
-  O::mul(aT3, aT2, aT1);           // H^3
-  O::mul(aT2, aT2, aX);            // X H^2
-  O::sqr(aX, aT0);
-  O::sub(aX, aX, aT3);
-  O::sub(aX, aX, aT2);
-  O::sub(aX, aX, aT2);             // X3
-  O::sub(aT2, aT2, aX);
-  O::mul(aT2, aT2, aT0);
-  O::mul(aT3, aT3, aY);
-  O::sub(aY, aT2, aT3);            // Y3
-  O::sqr(aZ2, aZ);
-}
-
-// ---- the same two steps with five temporaries (aT0..aT4) -------------------------------------
-// Re-ordered so that aT5 is never touched: 13 slots instead of 14, which at 136 bytes per slot is
-// the difference between 96 and 128 threads per block for the 34-limb field (one warp per
-// scheduler instead of three warps on four).  Same operations, same values.
+// Five temporaries (aT0..aT4), aT5 is never touched: 13 slots instead of 14, which at 136 bytes per slot
+// is the difference between 96 and 128 threads per block for the 34-limb field (one warp per scheduler
+// instead of three warps on four).
 template <class O>
 PBC_STEP void a_double_step_5t() {
   // f = f^2
@@ -152,6 +73,14 @@ PBC_STEP void a_double_step_5t() {
   O::sub(aY, aY, aT1);             // Y' = M (S - X') - 8 Y^4
   a_fmul<O>(aF0, aF1, aT4, aT3, aT0, aT1, aT2);
 }
+// Chord through V = (X, Y, Z) (Jacobian, Z2 = Z^2) and the affine point P = (xP, yP), evaluated at
+// phi(Q); then V <- V + P.
+// Device replacement for compute_abc_line_proj + a_miller_evalfn + proj_add of a1_pairing_proj
+// (ecc/a_param.c:1820-1837, :306-315, :1869-1896); same line, same point, fewer products:
+//   H = xP Z^2 - X,  R = yP Z^3 - Y
+//   a = -R,  b = H Z (= Z of the sum),  c = yP Z X - xP Y;   l(phi(Q)) = (c - a Qx) + i (b Qy)
+//   X3 = R^2 - H^3 - 2 X H^2,  Y3 = R (X H^2 - X3) - Y H^3,  Z3 = b
+// 16 multiplications + 3 squarings including the f update.  Temporaries aT0..aT4 and aZ2.
 // P is fetched through `ldP(slot, coordinate)` (0 = x, 1 = y) when it is needed: x into aT4, y into
 // the Z^2 slot once Z^2 has had its last use; the point addition is finished before the f update
 // so that the update finds three free temporaries.

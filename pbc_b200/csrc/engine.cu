@@ -151,17 +151,13 @@ struct pbc_b200_pairing_s {
   AConsts a;
   A1Consts a1;
   A1GroupConsts a1g;
-#if PBC_A1_NAF
   A1Naf a1naf;
-#endif
   size_t a1_rows = 0;          // rows of the fixed-argument line table (3 per tangent / chord)
   EConsts e;                   // type e (also uses fp, a1.wb and a1g.n / zlen: the 34-limb pieces of type a1)
   uint32_t e_pts[4 * kNA1];    // a, b, x(R), y(R), Montgomery form (g_e_pts)
   size_t cc_rows = 0;          // types f, d, g: lines of the Miller walk (computed once at init)
   CCConsts cc;
-#if PBC_CC_NAF
   CCNaf ccnaf;
-#endif
   FConsts f;
   DConsts d;
   // type d with 160..255-bit q: the eight-limb instance (engine_d_wide.cu) and its constants; fp and
@@ -171,9 +167,7 @@ struct pbc_b200_pairing_s {
   DConstsT<pbcb200_dw::kLimbs> dw_d;
   ZrConstsT<pbcb200_dw::kLimbs> dw_zr;
   FqWideConstsT<pbcb200_dw::kLimbs> dw_x;
-#if PBC_CC_NAF
   CCNaf dw_naf;
-#endif
   GConsts g;
   ZrConsts zr;
   HashConsts hash;
@@ -207,7 +201,7 @@ static constexpr int kBlockMiller = 128;
 static constexpr int kBlockFinal = 128;
 static constexpr int kBlockInv = 128;
 static constexpr int kBlockCC = 128;           // types f, d: threads per block
-static constexpr int kBlockCCMiller = PBC_CC_MILLER_BLOCK;   // ... of the Miller kernels (lock-step barrier)
+static constexpr int kBlockCCMiller = kCCMillerBlock;   // ... of the Miller kernels (lock-step barrier)
 
 // The three reference operations that reach the GPU (include/pbc_pairing.h:141-171, :54-89).
 enum Mode { kSingle = 0, kProd = 1, kPP = 2 };
@@ -267,14 +261,9 @@ static size_t cc_table_rows_compute(const pbc_b200_pairing_s* p) {
   BigUInt r;
   if (p->dwide) for (int i = pbcb200_dw::kLimbs; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->dw_cc.r[i]);
   else for (int i = kNS; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->cc.r[i]);
-#if PBC_CC_NAF
   std::vector<int8_t> dg = naf_digits(r);
   size_t rows = dg.size() - 1;
   for (size_t m = 1; m + 1 < dg.size(); m++) rows += dg[m] ? 1 : 0;
-#else
-  size_t rows = r.bits() - 1;
-  for (size_t m = 1; m + 1 < r.bits(); m++) rows += r.bit(m) ? 1 : 0;
-#endif
   return rows;
 }
 static size_t cc_table_rows(const pbc_b200_pairing_s* p) { return p->cc_rows; }
@@ -299,16 +288,6 @@ static void fill_fp_consts(FpConsts* c, const BigUInt& q, int nlimbs) {
   (q - BigUInt(2)).to_words(c->pm2, nlimbs);
   c->np0 = neg_inv32(q.word(0));
   c->nlimbs = (uint32_t)nlimbs;
-  if (nlimbs == kNS) {
-    // -q^-1 mod 2^160 by Newton iteration x <- x (2 - q x): each step doubles the number of correct low bits
-    BigUInt R5 = BigUInt(1).shl(160), x(1), two(2);
-    for (int it = 0; it < 9; it++) {
-      BigUInt qx = (q * x) % R5;
-      BigUInt f = (two + R5 - qx) % R5;                 // 2 - q x mod 2^160
-      x = (x * f) % R5;
-    }
-    ((R5 - x) % R5).to_words(c->ninv, 5);
-  }
 }
 
 static bool get_big(const std::map<std::string, std::string>& tab, const char* key, BigUInt* out) {
@@ -401,7 +380,6 @@ static int init_type_a1(pbc_b200_pairing_s* p, const std::map<std::string, std::
   gc.expbits = (uint32_t)se.bits();
   gc.zlen = p->zr.zlen;
   gc.count = (uint32_t)wb;
-#if PBC_A1_NAF
   {
     std::vector<int8_t> dg = naf_digits(n);
     if (dg.size() > 32 * (size_t)kMaxLimbs) return fail("type a1: n too large for the signed-digit table");
@@ -412,7 +390,6 @@ static int init_type_a1(pbc_b200_pairing_s* p, const std::map<std::string, std::
     }
     p->a1naf.len = (uint32_t)dg.size();
   }
-#endif
   p->hash_ok = false;
   return 0;
 }
@@ -650,7 +627,7 @@ static int init_type_f(pbc_b200_pairing_s* p, const std::map<std::string, std::s
 // upper end is where the eight-limb code stops being exact, the least of:
 //   * mont_mul<8, false>, fp_add<8, false>, fp_halve (FULL = false, no carry word): a + q <= 2^256 for the
 //     operands they see, all canonical (< q): q < 2^255;
-//   * the lazy F_q^3 product (pairing_d.cuh, PBC_D_LAZY, internal basis): fq_add_nr sums below 2q < 2^256
+//   * the lazy F_q^3 product (pairing_d.cuh, internal basis): fq_add_nr sums below 2q < 2^256
 //     fit the limbs, every value handed to the reduction lies in (0, 4 q^2), and redc_wide takes t < 2 q R:
 //     4 q^2 < 2 q 2^256, again q < 2^255;
 //   * fq_from_wire: any 32-byte input is below R and mont_mul_ps(x, R^2 mod q) of it is below 2q: q < 2^255;
@@ -787,7 +764,6 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
     to_mont(p->dw_x.ts_c, BigUInt::powmod(z, Q, q), q, NW);
     p->derived["sqrt_nonresidue"] = {z};
   }
-#if PBC_CC_NAF
   {
     std::vector<int8_t> dg = naf_digits(r);
     memset(&p->dw_naf, 0, sizeof p->dw_naf);
@@ -797,7 +773,6 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
     }
     p->dw_naf.len = (uint32_t)dg.size();
   }
-#endif
   return fill_type_d<NW>(p, p->dw_d, q, r, a, b, nqr, c0, c1, c2);
 }
 
@@ -1033,17 +1008,11 @@ static cudaError_t allow_smem(K kernel, size_t bytes) {
 }
 
 static constexpr size_t kSmemAMiller9 = (size_t)kA9Slots * 64 * kBlockMiller;
-// PBC_F_SLOTS = 1 (default): type F Miller loop on the shared-memory slot machine (pairing_f_slots.cuh)
-// where the parameters allow it; 0: the round-1 kernel (local-memory frames)
-#ifndef PBC_F_SLOTS
-#define PBC_F_SLOTS 1
-#endif
+// type F on the shared-memory slot machine (pairing_f_slots.cuh) where the parameters allow it, else the
+// round-1 kernels (local-memory frames)
 static constexpr int kBlockFS = 128;
-// threads per block of the slot-machine Miller kernel: 128 -> two blocks (8 warps) per SM, 96 -> three blocks (9 warps)
-#ifndef PBC_FS_MILLER_BLOCK
-#define PBC_FS_MILLER_BLOCK 128
-#endif
-static constexpr int kBlockFSM = PBC_FS_MILLER_BLOCK;
+// threads per block of the slot-machine Miller kernel: 128 -> two blocks (8 warps) per SM
+static constexpr int kBlockFSM = 128;
 static constexpr size_t kSmemFMillerS = (size_t)kFSlots * kNS * 4 * kBlockFSM;
 static constexpr size_t kSmemFFinalS = (size_t)kFFinalSlots * kNS * 4 * kBlockFS;
 static constexpr size_t kSmemAFinal = (size_t)kAFSlots * 64 * kBlockFinal;
@@ -1054,7 +1023,7 @@ static constexpr size_t kSmemAPPInit = (size_t)kASlots * 64 * 32;
 static constexpr size_t kSmemAPPApply = (size_t)kAPPSlots * 64 * kBlockMiller;
 
 // type a1: 34-limb slots (136 bytes per thread and slot)
-static constexpr int kBlockA1 = kA1MillerBlock;  // 14 slots * 136 B * 96 threads = 178.5 KB of shared memory (13 * 136 * 128 = 221 KB with PBC_A1_SLOTS13)
+static constexpr int kBlockA1 = kA1MillerBlock;  // 13 slots * 136 B * 128 threads = 221 KB of shared memory
 static constexpr int kBlockA1Small = 128;      // kernels with at most 9 slots
 static constexpr size_t kSlotA1 = (size_t)kNA1 * 4;
 static constexpr size_t kSmemA1Miller = (size_t)kA1MillerSlots * kSlotA1 * kBlockA1;
@@ -1136,15 +1105,8 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
   std::lock_guard<std::mutex> lk(g_const_mu);
   if (g_const_owner[dev] != p->id && p->dwide) {
     CUDA_OK(cudaDeviceSynchronize());
-#if PBC_CC_NAF
-    const void* naf = &p->dw_naf;
-    const size_t naf_bytes = sizeof p->dw_naf;
-#else
-    const void* naf = nullptr;
-    const size_t naf_bytes = 0;
-#endif
-    pbcb200_dw::DWideConsts w = {&p->fp, &p->dw_cc, naf, &p->dw_d, &p->dw_zr, &p->hash, &p->dw_x,
-                                 sizeof p->fp, sizeof p->dw_cc, naf_bytes, sizeof p->dw_d, sizeof p->dw_zr,
+    pbcb200_dw::DWideConsts w = {&p->fp, &p->dw_cc, &p->dw_naf, &p->dw_d, &p->dw_zr, &p->hash, &p->dw_x,
+                                 sizeof p->fp, sizeof p->dw_cc, sizeof p->dw_naf, sizeof p->dw_d, sizeof p->dw_zr,
                                  sizeof p->hash, sizeof p->dw_x};
     const int e = pbcb200_dw::dw_upload(w);
     if (e == -2) return fail("type d: this build has no eight-limb instance (160..255-bit q)");
@@ -1165,13 +1127,10 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
       CUDA_OK(cudaMemcpyToSymbol(c_e, &p->e, sizeof(EConsts)));
       CUDA_OK(cudaMemcpyToSymbol(g_e_pts, p->e_pts, sizeof p->e_pts));
     }
-#if PBC_A1_NAF
     if (p->type == '1') CUDA_OK(cudaMemcpyToSymbol(c_a1naf, &p->a1naf, sizeof(A1Naf)));
-#endif
     CUDA_OK(cudaMemcpyToSymbol(c_zr, &p->zr, sizeof(ZrConsts)));
     CUDA_OK(cudaMemcpyToSymbol(c_hash, &p->hash, sizeof(HashConsts)));
     if (p->type == 'f' || p->type == 'd' || p->type == 'g') CUDA_OK(cudaMemcpyToSymbol(c_cc, &p->cc, sizeof(CCConsts)));
-#if PBC_CC_NAF
     if (p->type == 'f' || p->type == 'd' || p->type == 'g') {
       // signed digits of the group order (host_naf.hpp); r is what fill_cc stored
       BigUInt r;
@@ -1185,7 +1144,6 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
       p->ccnaf.len = (uint32_t)dg.size();
       CUDA_OK(cudaMemcpyToSymbol(c_ccnaf, &p->ccnaf, sizeof(CCNaf)));
     }
-#endif
     if (p->type == 'f') CUDA_OK(cudaMemcpyToSymbol(c_f, &p->f, sizeof(FConsts)));
     if (p->type == 'd') CUDA_OK(cudaMemcpyToSymbol(c_d, &p->d, sizeof(DConsts)));
     if (p->type == 'g') CUDA_OK(cudaMemcpyToSymbol(c_g, &p->g, sizeof(GConsts)));
@@ -1439,7 +1397,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       }
     }
     if (wide) pbcb200_dw::dw_miller(d_in1, d_in2, mv, flag, m, stride1, tab, rows, st);
-    else if (isf && PBC_F_SLOTS && p->f.slots_ok) {
+    else if (isf && p->f.slots_ok) {
       uint32_t* gq = mv + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0);   // after the Miller values and flags
       k_f_miller_s<kBlockFSM><<<(unsigned)((m + kBlockFSM - 1) / kBlockFSM), kBlockFSM, kSmemFMillerS, st>>>(d_in1, d_in2, mv, flag, gq, m, stride1, tab, rows);
     } else if (isf) k_f_miller<kBlockCCMiller><<<gm, kBlockCCMiller, 0, st>>>(d_in1, d_in2, mv, flag, m, stride1, tab, rows);
@@ -1462,7 +1420,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     unsigned gf = (unsigned)((n + kBlockCC - 1) / kBlockCC);
     unsigned gfm = (unsigned)((n + kBlockCCMiller - 1) / kBlockCCMiller);
     if (wide) pbcb200_dw::dw_finalexp(mv, flag, d_out, n, st);
-    else if (isf && PBC_F_SLOTS && p->f.slots_ok && p->f.bn) {
+    else if (isf && p->f.slots_ok && p->f.bn) {
       uint32_t* stash = (uint32_t*)ws + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0) + (size_t)kFGWords * m;
       k_f_finalexp_s<kBlockFS><<<(unsigned)((n + kBlockFS - 1) / kBlockFS), kBlockFS, kSmemFFinalS, st>>>(mv, flag, d_out, stash, n);
     } else if (isf) k_f_finalexp<kBlockCCMiller><<<gfm, kBlockCCMiller, 0, st>>>(mv, flag, d_out, n);

@@ -6,7 +6,7 @@
 // so that the kernels and the __constant__ symbols of the two instances never meet: the five-limb
 // kernels compile exactly as before.  Differences of this instance, all selected at compile time:
 //   * the wire width ceil(bits(q)/8) (22 .. 32 bytes) is a run-time constant (c_fqx.wb);
-//   * single products are mont_mul<8, false>, the lazy F_q^3 product (PBC_D_LAZY) uses the double-width
+//   * single products are mont_mul<8, false>, the lazy F_q^3 product uses the double-width
 //     product and reduction of fp.cuh (mul_wide<8>, redc_wide<8>);
 //   * scalars have eight words (r < 2^255);
 //   * q = 1 mod 8 takes Tonelli-Shanks square roots (element_from_hash, compressed points).
@@ -26,27 +26,20 @@
 
 namespace pbcb200 {
 
-static constexpr int kBlockWMiller = PBC_CC_MILLER_BLOCK;   // as engine.cu's type D kernels
+static constexpr int kBlockWMiller = kCCMillerBlock;   // as engine.cu's type D kernels
 static constexpr int kBlockW = 128;
 
 static unsigned grid(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
 
 int dw_upload(const DWideConsts& c) {
-#if PBC_CC_NAF
-  const size_t naf_bytes = sizeof(CCNaf);
-#else
-  const size_t naf_bytes = 0;
-#endif
-  if (c.fp_bytes != sizeof(FpConsts) || c.cc_bytes != sizeof(CCConsts) || c.naf_bytes != naf_bytes ||
+  if (c.fp_bytes != sizeof(FpConsts) || c.cc_bytes != sizeof(CCConsts) || c.naf_bytes != sizeof(CCNaf) ||
       c.d_bytes != sizeof(DConsts) || c.zr_bytes != sizeof(ZrConsts) || c.hash_bytes != sizeof(HashConsts) ||
       c.x_bytes != sizeof(FqWideConstsT<kNS>))
     return -1;
   cudaError_t e;
   if ((e = cudaMemcpyToSymbol(c_fp, c.fp, c.fp_bytes)) != cudaSuccess) return e;
   if ((e = cudaMemcpyToSymbol(c_cc, c.cc, c.cc_bytes)) != cudaSuccess) return e;
-#if PBC_CC_NAF
   if ((e = cudaMemcpyToSymbol(c_ccnaf, c.naf, c.naf_bytes)) != cudaSuccess) return e;
-#endif
   if ((e = cudaMemcpyToSymbol(c_d, c.d, c.d_bytes)) != cudaSuccess) return e;
   if ((e = cudaMemcpyToSymbol(c_zr, c.zr, c.zr_bytes)) != cudaSuccess) return e;
   if ((e = cudaMemcpyToSymbol(c_hash, c.hash, c.hash_bytes)) != cudaSuccess) return e;

@@ -29,8 +29,8 @@ struct FpConsts {
   uint32_t pm2[kMaxLimbs];   // p - 2       (Fermat inversion exponent)
   uint32_t np0;              // -p^-1 mod 2^32
   uint32_t nlimbs;
-  uint32_t pad[2];
-  uint32_t ninv[8];          // -p^-1 mod 2^160 (five-limb fields: the two-product Montgomery reduction fqw_redc_split)
+  uint32_t pad[10];          // 8 words more than alignment needs: they keep c_fp at its size, so the constant-bank
+                             // offsets of every later __constant__ symbol (and with them most kernels' code) stay put
 };
 
 __constant__ FpConsts c_fp;   // single translation unit (engine.cu)
@@ -423,26 +423,14 @@ __device__ __forceinline__ void mont_sqr_ps(uint32_t* r, const uint32_t* a) {
 // The multiplier the kernels use.  Where IMAD.WIDE.U32 issues at the same rate with or without
 // carries, the two multipliers execute the same number of multiplier-pipe slots; operand scanning has
 // about a quarter fewer ALU instructions and suits a*b, product scanning suits a^2 (408 instead of 528
-// IMAD.WIDE).  PBC_MULT_IMPL: 2 = that hybrid (default), 1 = product scanning for both, 0 = operand
-// scanning for both.
-#ifndef PBC_MULT_IMPL
-#define PBC_MULT_IMPL 2
-#endif
+// IMAD.WIDE): operand scanning for products, product scanning for squares.
 template <int N, bool FULL>
 __device__ __forceinline__ void fp_mul(uint32_t* r, const uint32_t* a, const uint32_t* b) {
-#if PBC_MULT_IMPL == 1
-  mont_mul_ps<N, FULL>(r, a, b);
-#else
   mont_mul<N, FULL>(r, a, b);
-#endif
 }
 template <int N, bool FULL>
 __device__ __forceinline__ void fp_sqr(uint32_t* r, const uint32_t* a) {
-#if PBC_MULT_IMPL >= 1
   mont_sqr_ps<N, FULL>(r, a);
-#else
-  mont_mul<N, FULL>(r, a, a);
-#endif
 }
 
 // ---------------------------------------------------------------------------------------------

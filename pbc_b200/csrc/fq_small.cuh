@@ -15,9 +15,7 @@
 
 namespace pbcb200 {
 
-// PBC_NS: 32-bit limbs of the small field.  5 = minimal (product-scanning multiplier, 55 products,
-// ~140 instructions); 6 = one spare limb so the even/odd operand-scanning multiplier of fp.cuh applies
-// (78 products but ~105 instructions) -- an A/B experiment, see DESIGN.md.
+// PBC_NS: 32-bit limbs of the small field: 5 here, 8 in the wide instance below.
 // PBC_FQ_WIDE = 1: the eight-limb instance of type D for 160- to 255-bit q (engine_d_wide.cu, its own
 // translation unit and namespace): the wire width is a run-time constant there, and q = 1 mod 8 takes
 // Tonelli-Shanks square roots.
@@ -53,68 +51,29 @@ __device__ __forceinline__ int wire_w() { return W ? W : fq_wb(); }
 
 struct Fq { uint32_t v[kNS]; };
 
-// PBC_FQ_CALL = 1: one out-of-line copy of the multiplier and of the squarer, operands and result
-// by value (five registers each way).  The tower routines contain dozens of products; fully inlined
-// they outgrow the instruction cache (instruction fetch becomes the top stall of k_d_miller).
-#ifndef PBC_FQ_CALL
-#define PBC_FQ_CALL 1
-#endif
-// PBC_FQ_CALL_OS: the out-of-line multiplier is the row-wise product + row-wise reduction (fq_mul_os below: 55
-// products, about 100 instructions) instead of the column-wise one (50 products, about 150 instructions);
-// 2 = the squarer too (55 instead of 40 products).  a b < q R is all it needs (operands below 2q and q).
-#ifndef PBC_FQ_CALL_OS
-#define PBC_FQ_CALL_OS 1
-#endif
+// One out-of-line copy of the multiplier and of the squarer, operands and result by value (five
+// registers each way).  The tower routines contain dozens of products; fully inlined they outgrow the
+// instruction cache (instruction fetch becomes the top stall of k_d_miller).  The five-limb multiplier is
+// the row-wise product + row-wise reduction (fq_mul_os below: 55 products, about 100 instructions; a b < q R
+// is all it needs, operands below 2q and q), the squarer the column-wise one of fp.cuh (40 products).
 __device__ __forceinline__ void fq_mul_os(Fq& r, const Fq& a, const Fq& b);
-#if PBC_FQ_CALL
 __device__ __noinline__ Fq fq_mul_call(Fq a, Fq b) {
   Fq r;
   if constexpr (kNS % 2 == 0) mont_mul<kNS + (kNS & 1), false>(r.v, a.v, b.v);
-  else if (PBC_FQ_CALL_OS) fq_mul_os(r, a, b);
-  else mont_mul_ps<kNS, false>(r.v, a.v, b.v);
+  else fq_mul_os(r, a, b);
   return r;
 }
 __device__ __noinline__ Fq fq_sqr_call(Fq a) {
   Fq r;
   if constexpr (kNS % 2 == 0) mont_mul<kNS + (kNS & 1), false>(r.v, a.v, a.v);
-  else if (PBC_FQ_CALL_OS >= 2) fq_mul_os(r, a, a);
   else mont_sqr_ps<kNS, false>(r.v, a.v);
   return r;
 }
 __device__ __forceinline__ void fq_mul(Fq& r, const Fq& a, const Fq& b) { r = fq_mul_call(a, b); }
 __device__ __forceinline__ void fq_sqr(Fq& r, const Fq& a) { r = fq_sqr_call(a); }
-// the hottest tower routines (F_q^2 / F_q^3 products) may still inline their few products: one
-// copy each, no argument shuffling (PBC_HOT_INLINE)
-#ifndef PBC_HOT_INLINE
-#define PBC_HOT_INLINE 0
-#endif
-__device__ __forceinline__ void fq_mul_hot(Fq& r, const Fq& a, const Fq& b) {
-  if (PBC_HOT_INLINE) mont_mul_ps<kNS, false>(r.v, a.v, b.v); else r = fq_mul_call(a, b);
-}
-__device__ __forceinline__ void fq_sqr_hot(Fq& r, const Fq& a) {
-  if (PBC_HOT_INLINE) mont_sqr_ps<kNS, false>(r.v, a.v); else r = fq_sqr_call(a);
-}
-#else
-__device__ __forceinline__ void fq_mul_hot(Fq& r, const Fq& a, const Fq& b) { mont_mul_ps<kNS, false>(r.v, a.v, b.v); }
-__device__ __forceinline__ void fq_sqr_hot(Fq& r, const Fq& a) { mont_sqr_ps<kNS, false>(r.v, a.v); }
-__device__ __forceinline__ void fq_mul(Fq& r, const Fq& a, const Fq& b) { mont_mul_ps<kNS, false>(r.v, a.v, b.v); }
-__device__ __forceinline__ void fq_sqr(Fq& r, const Fq& a) { mont_sqr_ps<kNS, false>(r.v, a.v); }
-#endif
-// PBC_FQ_ADD_CALL = 1: additions and subtractions out of line as well (code size experiment)
-#ifndef PBC_FQ_ADD_CALL
-#define PBC_FQ_ADD_CALL 0
-#endif
-__device__ __noinline__ Fq fq_add_call(Fq a, Fq b) { Fq r; fp_add<kNS, false>(r.v, a.v, b.v); return r; }
-__device__ __noinline__ Fq fq_sub_call(Fq a, Fq b) { Fq r; fp_sub<kNS>(r.v, a.v, b.v); return r; }
-#if PBC_FQ_ADD_CALL
-__device__ __forceinline__ void fq_add(Fq& r, const Fq& a, const Fq& b) { r = fq_add_call(a, b); }
-__device__ __forceinline__ void fq_sub(Fq& r, const Fq& a, const Fq& b) { r = fq_sub_call(a, b); }
-__device__ __forceinline__ void fq_dbl(Fq& r, const Fq& a) { r = fq_add_call(a, a); }
-#else
 __device__ __forceinline__ void fq_add(Fq& r, const Fq& a, const Fq& b) { fp_add<kNS, false>(r.v, a.v, b.v); }
 __device__ __forceinline__ void fq_sub(Fq& r, const Fq& a, const Fq& b) { fp_sub<kNS>(r.v, a.v, b.v); }
 __device__ __forceinline__ void fq_dbl(Fq& r, const Fq& a) { fp_add<kNS, false>(r.v, a.v, a.v); }
-#endif
 __device__ __forceinline__ void fq_neg(Fq& r, const Fq& a) { fp_neg<kNS>(r.v, a.v); }
 __device__ __forceinline__ void fq_halve(Fq& r, const Fq& a) { fp_halve<kNS, false>(r.v, a.v); }
 __device__ __forceinline__ bool fq_is_zero(const Fq& a) { return fp_is_zero<kNS>(a.v); }
@@ -218,28 +177,17 @@ __device__ __forceinline__ void fqw_sub(FqW& r, const FqW& a, const FqW& b) {
 // The column-wise form this replaces (fq_mulw_call in fq_small.cuh) compiles to ~95 instructions per
 // product of two elements -- IMAD.WIDE + IADD3.X per product plus SEL / IMAD.MOV / IMAD.X to move
 // carries and re-align register pairs at every column, and those moves take multiplier-pipe slots; this one to ~40.
-#ifndef PBC_FQW_OS
-#define PBC_FQW_OS 1
-#endif
 #define PBC_MADW_FIRST(lo, hi, x, y) PBC_ASM("mad.lo.cc.u32 %0, %2, %3, %0; madc.hi.cc.u32 %1, %2, %3, %1;" : "+r"(lo), "+r"(hi) : "r"(x), "r"(y))
 #define PBC_MADW_NEXT(lo, hi, x, y) PBC_ASM("madc.lo.cc.u32 %0, %2, %3, %0; madc.hi.cc.u32 %1, %2, %3, %1;" : "+r"(lo), "+r"(hi) : "r"(x), "r"(y))
 // (lo, hi) = x y.  Written as a multiply-add of zero: ptxas turns mad.lo.cc + madc.hi into ONE IMAD.WIDE.U32, while
 // mul.lo + mul.hi stayed an IMAD + IMAD.HI pair in places.  Clobbers the carry flag (no run is in flight where a
 // row starts).  Tiling the accumulators with nine plain products first, to avoid the "(carry word, 0)" top pairs and
 // their zeroing moves, did not pay: ptxas moved other additions onto the multiplier pipe instead (IMAD.X / IMAD).
-#ifndef PBC_MULW_MAD
-#define PBC_MULW_MAD 1
-#endif
-#if PBC_MULW_MAD
 #define PBC_MULW_PAIR(lo, hi, x, y) PBC_ASM("mad.lo.cc.u32 %0, %2, %3, 0; madc.hi.u32 %1, %2, %3, 0;" : "=r"(lo), "=r"(hi) : "r"(x), "r"(y))
-#else
-#define PBC_MULW_PAIR(lo, hi, x, y) PBC_ASM("mul.lo.u32 %0, %2, %3; mul.hi.u32 %1, %2, %3;" : "=r"(lo), "=r"(hi) : "r"(x), "r"(y))
-#endif
 #define PBC_CARRY_TO(w) PBC_ASM("addc.u32 %0, 0, 0;" : "=r"(w))
 #if PBC_NS == 5
 __device__ __forceinline__ void fqw_mul(FqW& t, const Fq& a, const Fq& b) {
   static_assert(kNS == 5, "the row schedule below is written out for five limbs");
-#if PBC_FQW_OS
   uint32_t E[10], O[10];
   const uint32_t* x = a.v;
   const uint32_t* y = b.v;
@@ -287,17 +235,6 @@ __device__ __forceinline__ void fqw_mul(FqW& t, const Fq& a, const Fq& b) {
 #pragma unroll
   for (int k = 2; k < 9; k++) PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(t.v[k]) : "r"(E[k]), "r"(O[k]));
   PBC_ASM("addc.u32 %0, %1, %2;" : "=r"(t.v[9]) : "r"(E[9]), "r"(O[9]));
-#else
-  uint32_t u0 = 0, u1 = 0, u2 = 0;
-#pragma unroll
-  for (int i = 0; i < 2 * kNS - 1; i++) {
-#pragma unroll
-    for (int j = (i < kNS ? 0 : i - kNS + 1); j <= (i < kNS ? i : kNS - 1); j++) PBC_MAC3(u0, u1, u2, a.v[j], b.v[i - j]);
-    t.v[i] = u0;
-    u0 = u1; u1 = u2; u2 = 0;
-  }
-  t.v[2 * kNS - 1] = u0;
-#endif
 }
 #else
 // any even limb count (the wide instance): the operand-scanning double-width product of fp.cuh
@@ -340,81 +277,6 @@ __device__ __forceinline__ void fqw_redc2(Fq& r, const FqW& t) {
 #pragma unroll
   for (int k = 0; k < kNS; k++) r.v[k] = borrow == 0 ? d[k] : o[k];
 }
-// ---------------------------------------------------------------------------------------------
-// Montgomery reduction as two products (PBC_FQW_REDC_SPLIT): m = (t mod R) (-q^-1) mod R -- the low half of
-// a 5 x 5 product, 10 full and 5 low-word products on the even / odd accumulators -- then u = m q (fqw_mul)
-// and r = (t + u) / R = t_hi + u_hi + (t_lo != 0).  40 products instead of 30, but no serial chain through
-// the five quotient digits: the column-wise fqw_redc2 computes each digit from the column sum the
-// previous digits feed, which is what a warp waits for when only two warps share a scheduler.
-// t < 2 q R as for fqw_redc2.
-// ---------------------------------------------------------------------------------------------
-#ifndef PBC_FQW_REDC_SPLIT
-#define PBC_FQW_REDC_SPLIT 0
-#endif
-__device__ __forceinline__ void fq_mullo(uint32_t* m, const uint32_t* x, const uint32_t* y) {
-  uint32_t E[5], O[5];
-  // row 0
-  PBC_MULW_PAIR(E[0], E[1], x[0], y[0]);
-  PBC_MULW_PAIR(E[2], E[3], x[2], y[0]);
-  E[4] = x[4] * y[0];
-  PBC_MULW_PAIR(O[1], O[2], x[1], y[0]);
-  PBC_MULW_PAIR(O[3], O[4], x[3], y[0]);
-  // row 1: even columns 2, 4 (low word only); odd columns 1, 3
-  PBC_MADW_FIRST(E[2], E[3], x[1], y[1]);
-  PBC_ASM("madc.lo.u32 %0, %1, %2, %0;" : "+r"(E[4]) : "r"(x[3]), "r"(y[1]));
-  PBC_MADW_FIRST(O[1], O[2], x[0], y[1]);
-  PBC_ASM("madc.lo.cc.u32 %0, %2, %3, %0; madc.hi.u32 %1, %2, %3, %1;" : "+r"(O[3]), "+r"(O[4]) : "r"(x[2]), "r"(y[1]));
-  // row 2: even columns 2, 4; odd column 3
-  PBC_MADW_FIRST(E[2], E[3], x[0], y[2]);
-  PBC_ASM("madc.lo.u32 %0, %1, %2, %0;" : "+r"(E[4]) : "r"(x[2]), "r"(y[2]));
-  PBC_ASM("mad.lo.cc.u32 %0, %2, %3, %0; madc.hi.u32 %1, %2, %3, %1;" : "+r"(O[3]), "+r"(O[4]) : "r"(x[1]), "r"(y[2]));
-  // row 3: even column 4; odd column 3
-  E[4] += x[1] * y[3];
-  PBC_ASM("mad.lo.cc.u32 %0, %2, %3, %0; madc.hi.u32 %1, %2, %3, %1;" : "+r"(O[3]), "+r"(O[4]) : "r"(x[0]), "r"(y[3]));
-  // row 4: even column 4
-  E[4] += x[0] * y[4];
-  m[0] = E[0];
-  PBC_ASM("add.cc.u32 %0, %1, %2;" : "=r"(m[1]) : "r"(E[1]), "r"(O[1]));
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(m[2]) : "r"(E[2]), "r"(O[2]));
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(m[3]) : "r"(E[3]), "r"(O[3]));
-  PBC_ASM("addc.u32 %0, %1, %2;" : "=r"(m[4]) : "r"(E[4]), "r"(O[4]));
-}
-__device__ __forceinline__ void fqw_redc_split(Fq& r, const FqW& t) {
-  Fq m, q;
-  FqW u;
-  fq_mullo(m.v, t.v, c_fp.ninv);
-  fq_set(q, c_fp.p);
-  fqw_mul(u, m, q);
-  // t_lo + u_lo is 0 or R: the carry into the high halves is (t_lo != 0)
-  uint32_t nz = t.v[0] | t.v[1] | t.v[2] | t.v[3] | t.v[4];
-  uint32_t o[kNS], top;
-  PBC_ASM("add.cc.u32 %0, %1, 0xffffffff;" : "=r"(top) : "r"(nz));          // carry flag = (nz != 0)
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(o[0]) : "r"(t.v[5]), "r"(u.v[5]));
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(o[1]) : "r"(t.v[6]), "r"(u.v[6]));
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(o[2]) : "r"(t.v[7]), "r"(u.v[7]));
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(o[3]) : "r"(t.v[8]), "r"(u.v[8]));
-  PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(o[4]) : "r"(t.v[9]), "r"(u.v[9]));
-  PBC_ASM("addc.u32 %0, 0, 0;" : "=r"(top));
-  // value = o + top 2^160 < 3 q: subtract q while it is >= q
-  uint32_t d[kNS], borrow;
-  PBC_ASM("sub.cc.u32 %0, %1, %2;" : "=r"(d[0]) : "r"(o[0]), "r"(c_fp.p[0]));
-#pragma unroll
-  for (int k = 1; k < kNS; k++) PBC_ASM("subc.cc.u32 %0, %1, %2;" : "=r"(d[k]) : "r"(o[k]), "r"(c_fp.p[k]));
-  PBC_ASM("subc.u32 %0, 0, 0;" : "=r"(borrow));
-  bool use_d = top != 0 || borrow == 0;
-#pragma unroll
-  for (int k = 0; k < kNS; k++) o[k] = use_d ? d[k] : o[k];
-  PBC_ASM("sub.cc.u32 %0, %1, %2;" : "=r"(d[0]) : "r"(o[0]), "r"(c_fp.p[0]));
-#pragma unroll
-  for (int k = 1; k < kNS; k++) PBC_ASM("subc.cc.u32 %0, %1, %2;" : "=r"(d[k]) : "r"(o[k]), "r"(c_fp.p[k]));
-  PBC_ASM("subc.u32 %0, 0, 0;" : "=r"(borrow));
-#pragma unroll
-  for (int k = 0; k < kNS; k++) r.v[k] = borrow == 0 ? d[k] : o[k];
-}
-// the reduction the slot-machine routines call
-__device__ __forceinline__ void fqw_reduce(Fq& r, const FqW& t) {
-  if (PBC_FQW_REDC_SPLIT) fqw_redc_split(r, t); else fqw_redc2(r, t);
-}
 
 // a + b without reduction (the caller knows the sum fits the limbs)
 __device__ __forceinline__ void fq_add_nr(Fq& r, const Fq& a, const Fq& b) {
@@ -424,7 +286,7 @@ __device__ __forceinline__ void fq_add_nr(Fq& r, const Fq& a, const Fq& b) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Accumulating products (PBC_FQ_ACC): sums of several 5 x 5 products kept UNMERGED on the even / odd
+// Accumulating products: sums of several 5 x 5 products kept UNMERGED on the even / odd
 // accumulators and merged once.  In the first slot kernels IADD3 outnumbered IMAD.WIDE in the instruction
 // stream -- every product paid a ten-word merge of its two accumulators plus one or two
 // ten-word additions into the running sums of an F_q^2 product, and the warps (two per scheduler) spent
@@ -436,9 +298,6 @@ __device__ __forceinline__ void fq_add_nr(Fq& r, const Fq& a, const Fq& b) {
 // a_1, a_3 on the other (words i+1 .. i+4); the carry out of either run is counted in K at the word
 // above the run.  The total stays below 2^320 (callers' bounds), so nothing is carried out of word 9.
 // ---------------------------------------------------------------------------------------------
-#ifndef PBC_FQ_ACC
-#define PBC_FQ_ACC 1
-#endif
 struct FqAcc { uint32_t E[10], O[10], K[5]; };
 
 #define PBC_CARRY_ADD(w) PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(w))

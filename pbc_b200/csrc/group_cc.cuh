@@ -19,7 +19,7 @@ namespace pbcb200 {
 
 // out[i] = k[i] * in[i] on y^2 = x^3 + A x + B over the five-limb field.  O -> zero bytes.
 template <int BLOCK, int W>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_cc_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_t* __restrict__ out,
             size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -134,7 +134,7 @@ __device__ __noinline__ void fq_sqrt_ts(Fq* out, const Fq* tp) {
 // square root (q = 3 mod 4: t^((q+1)/4); q = 5 mod 8: Atkin's b = (2t)^((q-5)/8), i = 2 t b^2,
 // root = t b (i - 1)), then the cofactor multiple (d159: h = 3; type f: none).
 template <int BLOCK, int W>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_cc_g1_from_hash(const uint8_t* __restrict__ data, int len, uint8_t* __restrict__ out, size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
@@ -257,7 +257,7 @@ k_cc_g1_from_hash(const uint8_t* __restrict__ data, int len, uint8_t* __restrict
 // element_from_bytes_compressed on G1 for the five-limb fields (ecc/curve.c:799-813): x (20 bytes) ||
 // sign byte -> x || y.  No square root -> zero bytes.
 template <int BLOCK, int W>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_cc_g1_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   if (idx >= n) return;
@@ -412,7 +412,7 @@ struct KF5 {                       // type g (19-byte coordinates)
 // out[i] = k[i] * in[i] on the twist.  One thread per point; all temporaries that are passed by
 // address live at function scope (stack discipline note in pairing_f.cuh).
 template <class KF, int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_t* __restrict__ out, size_t n) {
   typedef typename KF::El El;
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -495,7 +495,7 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
 #if !PBC_FQ_WIDE
 // out[i] = in[i]^k[i] in GT (type f: 240-byte F_q^12 elements)
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_f_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t* __restrict__ out,
            size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -520,7 +520,7 @@ k_f_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
 
 // type d: 120-byte F_q^6 elements
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_d_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t* __restrict__ out,
            size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -546,7 +546,7 @@ k_d_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
 #if !PBC_FQ_WIDE
 // type g: 190-byte F_q^10 elements
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_g_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t* __restrict__ out,
            size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;

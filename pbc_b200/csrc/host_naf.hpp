@@ -1,5 +1,5 @@
-// host_naf.hpp -- non-adjacent form of the group order, one-time host-side setup for the optional
-// signed-digit Miller loop of type A1 (PBC_A1_NAF).  The reference scans the plain bits of n
+// host_naf.hpp -- non-adjacent form of the group order, one-time host-side setup for the
+// signed-digit Miller loops (type A1; types F, D and G).  The reference scans the plain bits of n
 // ("TODO: sliding NAF", ecc/a_param.c:1978); a signed scan evaluates the same Miller function up to
 // vertical lines and constants in F_p^*, which the final exponentiation removes, with one chord per
 // three bits instead of one per two.  Shared with tests/host/a_steps_host.cpp.

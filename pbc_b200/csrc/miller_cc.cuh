@@ -16,22 +16,14 @@
 #pragma once
 #include "fq_small.cuh"
 
-// resident blocks per SM the F/D kernels are compiled for (caps registers at 65536 / (BLOCK * this))
-#ifndef PBC_CC_MINBLOCKS
-#define PBC_CC_MINBLOCKS 4
-#endif
-
-// PBC_CC_LOCKSTEP = 1: a block-wide barrier at the top of every Miller iteration keeps the warps of a
-// block in the same code region (the loop over the bits of r is uniform across pairings), so they
-// share instruction-cache lines; needs every thread of the block inside the loop.
-#ifndef PBC_CC_LOCKSTEP
-#define PBC_CC_LOCKSTEP 1
-#endif
-#ifndef PBC_CC_MILLER_BLOCK
-#define PBC_CC_MILLER_BLOCK 256
-#endif
-
 namespace pbcb200 {
+
+// resident blocks per SM the F/D kernels are compiled for (caps registers at 65536 / (BLOCK * this))
+constexpr int kCCMinBlocks = 4;
+// threads per block of the F/D/G Miller kernels.  A block-wide barrier at the top of every Miller iteration
+// keeps the warps of a block in the same code region (the loop over the digits of r is uniform across
+// pairings), so they share instruction-cache lines; every thread of the block has to run the loop.
+constexpr int kCCMillerBlock = 256;
 
 template <int NS>
 struct CCConstsT {
@@ -43,23 +35,17 @@ struct CCConstsT {
 typedef CCConstsT<kNS> CCConsts;
 __constant__ CCConsts c_cc;
 
-// PBC_CC_NAF = 1: the loop scans the non-adjacent form of r (host_naf.hpp) instead of its bits: one
-// chord + addition per three positions instead of one per two; where the digit is -1 the chord goes
-// through V and -P.  Vertical lines and constants lie in the subfield the final exponentiation
-// kills, so the reduced pairing is the same element (the reference keeps the plain scan).  Checked
-// bit for bit on the CPU simulator and by the GPU type F/D tests; faster for F, D and G (fewer chord steps);
-// the default.
-#ifndef PBC_CC_NAF
-#define PBC_CC_NAF 1
-#endif
-#if PBC_CC_NAF
+// The loop scans the non-adjacent form of r (host_naf.hpp) instead of its bits: one chord + addition
+// per three positions instead of one per two; where the digit is -1 the chord goes through V and -P.
+// Vertical lines and constants lie in the subfield the final exponentiation kills, so the reduced
+// pairing is the same element (the reference keeps the plain scan).  Faster for F, D and G (fewer
+// chord steps).
 struct CCNaf {
   uint32_t nz[8], neg[8];      // bit i: digit i non-zero / digit i is -1   (r below 2^255)
   uint32_t len;                // number of digits; the top one is +1
   uint32_t pad[3];
 };
 __constant__ CCNaf c_ccnaf;
-#endif
 
 // y^2 == x^3 + A x + B  (ecc/curve.c:57-76)
 __device__ __forceinline__ bool cc_on_curve(const Fq& x, const Fq& y) {
@@ -77,17 +63,6 @@ __device__ __forceinline__ bool cc_on_curve(const Fq& x, const Fq& y) {
 // T supplies:  struct Acc;  struct Ctx;
 //   static void mul_line(Acc* v, const Fq* a, const Fq* b, const Fq* c, const Ctx* ctx);   v *= line
 //   static void sqr(Acc* v);                                                               v  = v^2
-// PBC_CC_BODY_CALLS = 1 routes the additions of the loop body through out-of-line copies (smaller
-// body); slightly slower, so off
-#ifndef PBC_CC_BODY_CALLS
-#define PBC_CC_BODY_CALLS 0
-#endif
-__device__ __forceinline__ void mc_add(Fq& r, const Fq& a, const Fq& b) {
-  if (PBC_CC_BODY_CALLS) r = fq_add_call(a, b); else fq_add(r, a, b);
-}
-__device__ __forceinline__ void mc_sub(Fq& r, const Fq& a, const Fq& b) {
-  if (PBC_CC_BODY_CALLS) r = fq_sub_call(a, b); else fq_sub(r, a, b);
-}
 
 // The walk over the digits of r, generic in what happens to each line: `sink.line(a, b, c)` receives
 // the coefficients of every tangent and chord in loop order, `sink.sqr()` marks the squaring between
@@ -96,91 +71,79 @@ template <class Sink>
 __device__ __forceinline__ void miller_cc_walk(Sink& sink, const Fq& xP, const Fq& yP) {
   Fq X = xP, Y = yP, Z, a, b, c, M, Y2, Z2, t, u;
   fq_one(Z);
-#if PBC_CC_NAF
   int m = (int)c_ccnaf.len - 2;
   Fq yN;
   fq_neg(yN, yP);
-#else
-  int m = (int)c_cc.rbits - 2;
-#endif
   for (;;) {
-    if (PBC_CC_LOCKSTEP && Sink::kBarriers) __syncthreads();
+    if (Sink::kBarriers) __syncthreads();
     // ---- tangent at V ----
     fq_sqr(Z2, Z);
     fq_sqr(t, X);
-    mc_add(M, t, t);
-    mc_add(M, M, t);                       // 3 X^2
+    fq_add(M, t, t);
+    fq_add(M, M, t);                       // 3 X^2
     if (!c_cc.a_is_zero) {
       fq_sqr(u, Z2);
       fq_set(t, c_cc.A);
       fq_mul(u, u, t);
-      mc_add(M, M, u);                     // + A Z^4
+      fq_add(M, M, u);                     // + A Z^4
     }
     fq_sqr(Y2, Y);
     fq_mul(a, M, Z2);
     fq_neg(a, a);                          // a = -M Z^2
     fq_mul(u, Y, Z);
-    mc_add(u, u, u);                          // Z' = 2 Y Z
+    fq_add(u, u, u);                          // Z' = 2 Y Z
     fq_mul(b, u, Z2);                      // b = Z' Z^2
     fq_mul(c, M, X);
-    mc_sub(c, c, Y2);
-    mc_sub(c, c, Y2);                      // c = M X - 2 Y^2
+    fq_sub(c, c, Y2);
+    fq_sub(c, c, Y2);                      // c = M X - 2 Y^2
     sink.line(a, b, c);
     if (m == 0) break;
     // ---- V = 2 V ----
     fq_mul(t, X, Y2);
-    mc_add(t, t, t);
-    mc_add(t, t, t);                          // S = 4 X Y^2
+    fq_add(t, t, t);
+    fq_add(t, t, t);                          // S = 4 X Y^2
     Z = u;
     fq_sqr(X, M);
-    mc_sub(X, X, t);
-    mc_sub(X, X, t);                       // X' = M^2 - 2 S
+    fq_sub(X, X, t);
+    fq_sub(X, X, t);                       // X' = M^2 - 2 S
     fq_sqr(Y2, Y2);
-    mc_add(Y2, Y2, Y2);
-    mc_add(Y2, Y2, Y2);
-    mc_add(Y2, Y2, Y2);                        // 8 Y^4
-    mc_sub(t, t, X);
+    fq_add(Y2, Y2, Y2);
+    fq_add(Y2, Y2, Y2);
+    fq_add(Y2, Y2, Y2);                        // 8 Y^4
+    fq_sub(t, t, X);
     fq_mul(Y, M, t);
-    mc_sub(Y, Y, Y2);                      // Y' = M (S - X') - 8 Y^4
-#if PBC_CC_NAF
+    fq_sub(Y, Y, Y2);                      // Y' = M (S - X') - 8 Y^4
     if ((c_ccnaf.nz[m >> 5] >> (m & 31)) & 1u) {
       // ---- chord through V and +-P, then V = V +- P ----
       const Fq& yS = ((c_ccnaf.neg[m >> 5] >> (m & 31)) & 1u) ? yN : yP;
-#else
-    if ((c_cc.r[m >> 5] >> (m & 31)) & 1u) {
-      // ---- chord through V and P, then V = V + P ----
-      const Fq& yS = yP;
-#endif
       Fq H, R;
       fq_sqr(Z2, Z);
       fq_mul(t, Z2, Z);                    // Z^3
       fq_mul(H, xP, Z2);
-      mc_sub(H, H, X);                     // H = xP Z^2 - X
+      fq_sub(H, H, X);                     // H = xP Z^2 - X
       fq_mul(R, yS, t);
-      mc_sub(a, Y, R);                     // a = Y - yS Z^3
-      mc_sub(R, R, Y);                     // R = yP Z^3 - Y
+      fq_sub(a, Y, R);                     // a = Y - yS Z^3
+      fq_sub(R, R, Y);                     // R = yP Z^3 - Y
       fq_mul(b, H, Z);                     // b = H Z = Z of the sum
       fq_mul(t, yS, Z);
       fq_mul(t, t, X);
       fq_mul(u, xP, Y);
-      mc_sub(c, t, u);                     // c = yP Z X - xP Y
-      if (PBC_CC_LOCKSTEP >= 2 && Sink::kBarriers) __syncthreads();
+      fq_sub(c, t, u);                     // c = yP Z X - xP Y
       sink.line(a, b, c);
       fq_sqr(t, H);                        // H^2
       fq_mul(u, t, H);                     // H^3
       fq_mul(t, t, X);                     // X H^2
       fq_sqr(X, R);
-      mc_sub(X, X, u);
-      mc_sub(X, X, t);
-      mc_sub(X, X, t);                     // X3 = R^2 - H^3 - 2 X H^2
-      mc_sub(t, t, X);
+      fq_sub(X, X, u);
+      fq_sub(X, X, t);
+      fq_sub(X, X, t);                     // X3 = R^2 - H^3 - 2 X H^2
+      fq_sub(t, t, X);
       fq_mul(t, t, R);
       fq_mul(u, u, Y);
-      mc_sub(Y, t, u);                     // Y3 = R (X H^2 - X3) - Y H^3
+      fq_sub(Y, t, u);                     // Y3 = R (X H^2 - X3) - Y H^3
       Z = b;
     }
     m--;
-    if (PBC_CC_LOCKSTEP >= 2 && Sink::kBarriers) __syncthreads();
     sink.sqr();
   }
 }
@@ -243,22 +206,14 @@ __device__ __forceinline__ void miller_cc_tab(typename T::Acc* v, const uint32_t
                                               const typename T::Ctx* ctx) {
   Fq a, b, c;
   size_t row = 0;
-#if PBC_CC_NAF
   int m = (int)c_ccnaf.len - 2;
-#else
-  int m = (int)c_cc.rbits - 2;
-#endif
   for (;;) {
-    if (PBC_CC_LOCKSTEP) __syncthreads();
+    __syncthreads();
     fq_set(a, tab + (3 * row + 0) * kNS); fq_set(b, tab + (3 * row + 1) * kNS); fq_set(c, tab + (3 * row + 2) * kNS);
     row++;
     T::mul_line(v, &a, &b, &c, ctx);
     if (m == 0) break;
-#if PBC_CC_NAF
     if ((c_ccnaf.nz[m >> 5] >> (m & 31)) & 1u) {
-#else
-    if ((c_cc.r[m >> 5] >> (m & 31)) & 1u) {
-#endif
       fq_set(a, tab + (3 * row + 0) * kNS); fq_set(b, tab + (3 * row + 1) * kNS); fq_set(c, tab + (3 * row + 2) * kNS);
       row++;
       T::mul_line(v, &a, &b, &c, ctx);

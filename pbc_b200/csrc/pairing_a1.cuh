@@ -26,21 +26,13 @@ namespace pbcb200 {
 
 constexpr int kNA1 = 34;       // 32-bit limbs: p < 2^1087
 
-// PBC_A1_SLOTS13 = 1: Miller kernel on the five-temporary slot programs (13 slots, 128 threads per
-// block = one warp per scheduler) instead of 14 slots and 96 threads.  The programs are pinned on
-// the CPU (tests/test_a_steps_host.py, mode "5t").  A block of four warps takes about the time of a
-// block of three, so more pairings finish per SM; the default.
-#ifndef PBC_A1_SLOTS13
-#define PBC_A1_SLOTS13 1
-#endif
-// PBC_A1_NAF = 1: scan the non-adjacent form of n (host_naf.hpp) instead of its bits: a third fewer
-// chord steps (-11 % multiplier work for a1.param).  Pinned on the CPU (mode "naf" of the host
-// harness), bit-exact; the default.
-#ifndef PBC_A1_NAF
-#define PBC_A1_NAF 1
-#endif
-constexpr int kA1MillerSlots = PBC_A1_SLOTS13 ? 13 : 14;
-constexpr int kA1MillerBlock = PBC_A1_SLOTS13 ? 128 : 96;
+// The Miller kernel runs the five-temporary slot programs of a_steps.cuh: 13 slots, 128 threads per
+// block = one warp per scheduler (a block of four warps takes about the time of a block of three, so more
+// pairings finish per SM).  It scans the non-adjacent form of n (host_naf.hpp) instead of its bits: a
+// third fewer chord steps (-11 % multiplier work for a1.param).  Both are pinned on the CPU
+// (tests/test_a_steps_host.py).
+constexpr int kA1MillerSlots = 13;
+constexpr int kA1MillerBlock = 128;
 
 struct alignas(16) A1Consts {
   uint32_t n[kMaxLimbs];       // group order (plain integer, little-endian words)
@@ -52,7 +44,6 @@ struct alignas(16) A1Consts {
   uint32_t pad[3];
 };
 __constant__ A1Consts c_a1;
-#if PBC_A1_NAF
 struct alignas(16) A1Naf {
   uint32_t nz[kMaxLimbs];      // bit i: digit i is non-zero
   uint32_t neg[kMaxLimbs];     // bit i: digit i is -1
@@ -60,7 +51,6 @@ struct alignas(16) A1Naf {
   uint32_t pad[3];
 };
 __constant__ A1Naf c_a1naf;
-#endif
 
 // wire bytes (big-endian, wb per coordinate, any alignment) -> limbs
 __device__ __forceinline__ void a1_limbs_from_be(uint32_t* x, const uint8_t* p, int wb) {
@@ -144,51 +134,19 @@ k_a1_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, void* 
   O::set_const(aF0, c_fp.one);
   uint32_t zero[kNA1] = {0};
   O::st(aF1, zero);
-  // ecc/a_param.c:1979-1993: tangent; V = 2V; chord and V += P where the bit is set; f = f^2.
-  // a_double_step squares first, which is the same product because f starts at 1.
-#if !PBC_A1_NAF && !PBC_A1_SLOTS13
-  // the original configuration (kept textually apart from the variants below so that its
-  // generated code does not move when they change)
-  for (int m = (int)c_a1.nbits - 2; m >= 0; m--) {
-    a_double_step<O>();
-    if (m > 0 && ((c_a1.n[m >> 5] >> (m & 31)) & 1u)) {
-      O::ld_global(aT4, pm, 0, n, idx);
-      O::ld_global(aT5, pm, 1, n, idx);
-      a1_chord_add<O>(aT4, aT5);
-    }
-  }
-#else
-#if PBC_A1_NAF
+  // ecc/a_param.c:1979-1993: tangent; V = 2V; chord and V += P where the digit is non-zero; f = f^2.
+  // a_double_step_5t squares first, which is the same product because f starts at 1.
   const int top = (int)c_a1naf.len - 2;
-#else
-  const int top = (int)c_a1.nbits - 2;
-#endif
   for (int m = top; m >= 0; m--) {
-#if PBC_A1_NAF
     const bool chord = m > 0 && ((c_a1naf.nz[m >> 5] >> (m & 31)) & 1u);
     const bool minus = (c_a1naf.neg[m >> 5] >> (m & 31)) & 1u;      // V <- V - P: the chord through V and -P
-#else
-    const bool chord = m > 0 && ((c_a1.n[m >> 5] >> (m & 31)) & 1u);
-    const bool minus = false;
-#endif
-#if PBC_A1_SLOTS13
     a_double_step_5t<O>();
     if (chord)
       a1_chord_add_5t<O>([&](int slot, int coord) {
         O::ld_global(slot, pm, coord, n, idx);
         if (coord == 1 && minus) O::neg(slot, slot);
       });
-#else
-    a_double_step<O>();
-    if (chord) {
-      O::ld_global(aT4, pm, 0, n, idx);
-      O::ld_global(aT5, pm, 1, n, idx);
-      if (minus) O::neg(aT5, aT5);
-      a1_chord_add<O>(aT4, aT5);
-    }
-#endif
   }
-#endif
   a1_publish<O>(aF0, aF1, aT0, aT1, okP && okQ, f, dprod, n, idx);
 }
 

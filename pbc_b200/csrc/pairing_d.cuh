@@ -47,23 +47,8 @@ __constant__ DConsts c_d;
 // ---------------------------------------------------------------------------------------------
 // F_q^3
 // ---------------------------------------------------------------------------------------------
-// PBC_F3_ADD_CALL = 1 takes these out of line like PBC_F2_ADD_CALL in pairing_f.cuh; slower on type D
-// (the F_q^3 routines are smaller than F_q^12's), so they stay inline
-#ifndef PBC_F3_ADD_CALL
-#define PBC_F3_ADD_CALL 0
-#endif
-#if PBC_F3_ADD_CALL
-__device__ __noinline__ void f3_add_call(F3* r, const F3* x, const F3* y) {
-#pragma unroll
-  for (int i = 0; i < 3; i++) fq_add(r->c[i], x->c[i], y->c[i]);
-}
-__device__ __noinline__ void f3_sub_call(F3* r, const F3* x, const F3* y) {
-#pragma unroll
-  for (int i = 0; i < 3; i++) fq_sub(r->c[i], x->c[i], y->c[i]);
-}
-__device__ __forceinline__ void f3_add(F3& r, const F3& x, const F3& y) { f3_add_call(&r, &x, &y); }
-__device__ __forceinline__ void f3_sub(F3& r, const F3& x, const F3& y) { f3_sub_call(&r, &x, &y); }
-#else
+// The additions stay inline: out-of-line copies (as f2_add_call in pairing_f.cuh) were slower on type D,
+// whose F_q^3 routines are smaller than F_q^12's.
 __device__ __forceinline__ void f3_add(F3& r, const F3& x, const F3& y) {
 #pragma unroll
   for (int i = 0; i < 3; i++) fq_add(r.c[i], x.c[i], y.c[i]);
@@ -72,7 +57,6 @@ __device__ __forceinline__ void f3_sub(F3& r, const F3& x, const F3& y) {
 #pragma unroll
   for (int i = 0; i < 3; i++) fq_sub(r.c[i], x.c[i], y.c[i]);
 }
-#endif
 __device__ __forceinline__ void f3_neg(F3& r, const F3& x) {
 #pragma unroll
   for (int i = 0; i < 3; i++) fq_neg(r.c[i], x.c[i]);
@@ -101,10 +85,10 @@ __device__ __forceinline__ void f3_reduce(F3* r, const Fq& d0, const Fq& d1, con
   if (c_d.nice) {
     fq_set(k, c_d.pcoef);
     fq_sub(r->c[0], d0, d3);
-    fq_mul_hot(t, d3, k);
+    fq_mul(t, d3, k);
     fq_sub(r->c[1], d1, t);
     fq_sub(r->c[1], r->c[1], d4);
-    fq_mul_hot(t, d4, k);
+    fq_mul(t, d4, k);
     fq_sub(r->c[2], d2, t);
     return;
   }
@@ -112,10 +96,10 @@ __device__ __forceinline__ void f3_reduce(F3* r, const Fq& d0, const Fq& d1, con
   for (int i = 0; i < 3; i++) {
     const Fq& lo = i == 0 ? d0 : (i == 1 ? d1 : d2);
     fq_set(k, c_d.xpwr3[i]);
-    fq_mul_hot(t, d3, k);
+    fq_mul(t, d3, k);
     fq_add(r->c[i], lo, t);
     fq_set(k, c_d.xpwr4[i]);
-    fq_mul_hot(t, d4, k);
+    fq_mul(t, d4, k);
     fq_add(r->c[i], r->c[i], t);
   }
 }
@@ -155,44 +139,37 @@ __device__ __noinline__ void f3_to_reference(F3& v) {
   fq_mul(t, v.c[2], k);
   fq_sub(v.c[0], v.c[0], t);
 }
-// PBC_D_LAZY = 1 (internal basis only): the F_q^3 product and square keep their five partial
+// Internal basis only: the F_q^3 product and square keep their five partial
 // coefficients double width -- Karatsuba on unreduced 320-bit values, six fqw_mul -- reduce d3 and d4,
 // fold them with two more products by p and reduce three times: 8 x 25 + 5 x 30 = 350 multiplier
 // operations and 14 double-width additions instead of 8 Montgomery products (440) and 13 modular additions.
 //   w^3 = -p w - 1, w^4 = -p w^2 - w:   r0 = d0 - d3,  r1 = d1 - p d3 - d4,  r2 = d2 - p d4
 // with d1, d3 < 2 q^2, d2 < 3 q^2, d0, d4 < q^2; the offsets 2 q^2 / q^2 keep every value in (0, 4 q^2),
-// below the 2 q R that fqw_redc2 takes (2 q <= R for every q this build accepts).
-#ifndef PBC_D_LAZY
-#define PBC_D_LAZY 1
-#endif
-// the reduction of the lazy product: row-wise (fq_small.cuh, PBC_FQ_ACC) or column-wise
-__device__ __forceinline__ void fqw_reduce2(Fq& r, const FqW& t) {
-  if (PBC_FQ_ACC) fqw_redc_os<true>(r, t); else fqw_redc2(r, t);
-}
+// below the 2 q R that fqw_redc_os<true> takes (2 q <= R for every q this build accepts).
 __device__ __forceinline__ void f3_fold_lazy(F3* r, const FqW& d0, const FqW& d1, const FqW& d2, const FqW& d3,
                                              const FqW& d4) {
   Fq d3r, d4r, p;
   FqW w, t, q1, q2;
-  fqw_reduce2(d3r, d3);
-  fqw_reduce2(d4r, d4);
+  fqw_redc_os<true>(d3r, d3);
+  fqw_redc_os<true>(d4r, d4);
   fq_set(p, c_d.pcoef);
 #pragma unroll
   for (int k = 0; k < 2 * kNS; k++) { q1.v[k] = c_d.qsqm[0][k]; q2.v[k] = c_d.qsqm[1][k]; }
   fqw_add(w, d0, q2);
   fqw_sub(w, w, d3);
-  fqw_reduce2(r->c[0], w);
+  fqw_redc_os<true>(r->c[0], w);
   fqw_mul(t, p, d3r);
   fqw_add(w, d1, q2);
   fqw_sub(w, w, t);
   fqw_sub(w, w, d4);
-  fqw_reduce2(r->c[1], w);
+  fqw_redc_os<true>(r->c[1], w);
   fqw_mul(t, p, d4r);
   fqw_add(w, d2, q1);
   fqw_sub(w, w, t);
-  fqw_reduce2(r->c[2], w);
+  fqw_redc_os<true>(r->c[2], w);
 }
 __device__ __noinline__ void f3_mul(F3* r, const F3* x, const F3* y) {
-  if (PBC_D_LAZY && c_d.nice) {
+  if (c_d.nice) {
     const Fq x0 = x->c[0], x1 = x->c[1], x2 = x->c[2], y0 = y->c[0], y1 = y->c[1], y2 = y->c[2];
     Fq s, t;
     FqW d0, d1, d2, d3, d4, m1;
@@ -209,29 +186,29 @@ __device__ __noinline__ void f3_mul(F3* r, const F3* x, const F3* y) {
     return;
   }
   Fq d0, d1, d2, d3, d4, m1, s, t;
-  fq_mul_hot(d0, x->c[0], y->c[0]);
-  fq_mul_hot(m1, x->c[1], y->c[1]);
-  fq_mul_hot(d4, x->c[2], y->c[2]);
+  fq_mul(d0, x->c[0], y->c[0]);
+  fq_mul(m1, x->c[1], y->c[1]);
+  fq_mul(d4, x->c[2], y->c[2]);
   fq_add(s, x->c[0], x->c[1]);
   fq_add(t, y->c[0], y->c[1]);
-  fq_mul_hot(d1, s, t);
+  fq_mul(d1, s, t);
   fq_sub(d1, d1, d0);
   fq_sub(d1, d1, m1);
   fq_add(s, x->c[1], x->c[2]);
   fq_add(t, y->c[1], y->c[2]);
-  fq_mul_hot(d3, s, t);
+  fq_mul(d3, s, t);
   fq_sub(d3, d3, m1);
   fq_sub(d3, d3, d4);
   fq_add(s, x->c[0], x->c[2]);
   fq_add(t, y->c[0], y->c[2]);
-  fq_mul_hot(d2, s, t);
+  fq_mul(d2, s, t);
   fq_sub(d2, d2, d0);
   fq_sub(d2, d2, d4);
   fq_add(d2, d2, m1);
   f3_reduce(r, d0, d1, d2, d3, d4);
 }
 __device__ __noinline__ void f3_sqr(F3* r, const F3* x) {
-  if (PBC_D_LAZY && c_d.nice) {
+  if (c_d.nice) {
     const Fq x0 = x->c[0], x1 = x->c[1], x2 = x->c[2];
     FqW d0, d1, d2, d3, d4, w;
     fqw_mul(d0, x0, x0);
@@ -244,15 +221,15 @@ __device__ __noinline__ void f3_sqr(F3* r, const F3* x) {
     return;
   }
   Fq d0, d1, d2, d3, d4, t;
-  fq_sqr_hot(d0, x->c[0]);
-  fq_sqr_hot(d4, x->c[2]);
-  fq_mul_hot(d1, x->c[0], x->c[1]);
+  fq_sqr(d0, x->c[0]);
+  fq_sqr(d4, x->c[2]);
+  fq_mul(d1, x->c[0], x->c[1]);
   fq_dbl(d1, d1);
-  fq_mul_hot(d3, x->c[1], x->c[2]);
+  fq_mul(d3, x->c[1], x->c[2]);
   fq_dbl(d3, d3);
-  fq_mul_hot(d2, x->c[0], x->c[2]);
+  fq_mul(d2, x->c[0], x->c[2]);
   fq_dbl(d2, d2);
-  fq_sqr_hot(t, x->c[1]);
+  fq_sqr(t, x->c[1]);
   fq_add(d2, d2, t);
   f3_reduce(r, d0, d1, d2, d3, d4);
 }
@@ -367,7 +344,7 @@ __device__ __forceinline__ void f6d_ld_global(F6D& v, const uint32_t* g, size_t 
 // P: 40 bytes each (stride1 = 0 shares one P), Q: n x 120 bytes (x: 3 coefficients, y: 3).
 // tab != nullptr: the line coefficients of the (one) first argument come from the table (k_cc_pp_init).
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, (PBC_CC_MINBLOCKS * 128) / BLOCK)
+__global__ void __launch_bounds__(BLOCK, (kCCMinBlocks * 128) / BLOCK)
 k_d_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_t* __restrict__ mv,
            uint32_t* __restrict__ flag, size_t n, size_t stride1, const uint32_t* __restrict__ tab, size_t rows) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -421,7 +398,7 @@ k_d_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_
 
 // cc_pairings_affine (ecc/d_param.c:710-736): product of the k Miller values, one final power.
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_d_prod(const uint32_t* __restrict__ mv_in, const uint32_t* __restrict__ flag_in,
          uint32_t* __restrict__ mv_out, uint32_t* __restrict__ flag_out, size_t k, size_t n_out,
          size_t n_in) {
@@ -490,7 +467,7 @@ __device__ __noinline__ void f6d_final_exp(F3& out0, F3& out1, F6D& f) {
 // cc_tatepower, k = 6 branch (ecc/d_param.c:505-564) + lucas_even (:441-502).
 // out: n x 120 bytes: real half (3 coefficients) then imaginary half.
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_d_finalexp(const uint32_t* __restrict__ mv, const uint32_t* __restrict__ flag,
              uint8_t* __restrict__ out, size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;

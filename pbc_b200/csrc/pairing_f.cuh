@@ -62,21 +62,12 @@ __constant__ FConsts c_f;
 // F_q^2  (arith/fieldquadratic.c:197-309 fq_*)
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void f2_set(F2& r, const uint32_t c[2][kNS]) { fq_set(r.a, c[0]); fq_set(r.b, c[1]); }
-// PBC_F2_ADD_CALL = 1: one out-of-line copy of the F_q^2 addition and subtraction (the tower routines
-// contain dozens of them; inlined they make up most of f6_mul / f12_sqr and the kernels are
-// instruction-fetch bound at full occupancy)
-#ifndef PBC_F2_ADD_CALL
-#define PBC_F2_ADD_CALL 1
-#endif
-#if PBC_F2_ADD_CALL
+// one out-of-line copy of the F_q^2 addition and subtraction (the tower routines contain dozens of them;
+// inlined they make up most of f6_mul / f12_sqr and the kernels are instruction-fetch bound at full occupancy)
 __device__ __noinline__ void f2_add_call(F2* r, const F2* x, const F2* y) { fq_add(r->a, x->a, y->a); fq_add(r->b, x->b, y->b); }
 __device__ __noinline__ void f2_sub_call(F2* r, const F2* x, const F2* y) { fq_sub(r->a, x->a, y->a); fq_sub(r->b, x->b, y->b); }
 __device__ __forceinline__ void f2_add(F2& r, const F2& x, const F2& y) { f2_add_call(&r, &x, &y); }
 __device__ __forceinline__ void f2_sub(F2& r, const F2& x, const F2& y) { f2_sub_call(&r, &x, &y); }
-#else
-__device__ __forceinline__ void f2_add(F2& r, const F2& x, const F2& y) { fq_add(r.a, x.a, y.a); fq_add(r.b, x.b, y.b); }
-__device__ __forceinline__ void f2_sub(F2& r, const F2& x, const F2& y) { fq_sub(r.a, x.a, y.a); fq_sub(r.b, x.b, y.b); }
-#endif
 __device__ __forceinline__ void f2_dbl(F2& r, const F2& x) { fq_dbl(r.a, x.a); fq_dbl(r.b, x.b); }
 __device__ __forceinline__ void f2_neg(F2& r, const F2& x) { fq_neg(r.a, x.a); fq_neg(r.b, x.b); }
 __device__ __forceinline__ void f2_zero(F2& r) { fq_zero(r.a); fq_zero(r.b); }
@@ -84,14 +75,11 @@ __device__ __forceinline__ bool f2_eq(const F2& x, const F2& y) { return fq_eq(x
 
 // (x0 + x1 s)(y0 + y1 s) = x0 y0 + beta x1 y1 + ((x0 + x1)(y0 + y1) - x0 y0 - x1 y1) s;
 // internal basis: beta = -1, three multiplications.
-// Internal basis, lazily reduced (PBC_F2_LAZY): three unreduced products, the Karatsuba combination on
+// Internal basis, lazily reduced: three unreduced products, the Karatsuba combination on
 // double-width values, two reductions:  re = x0 y0 - x1 y1 + q^2 (< 2 q^2),  im = (x0 + x1)(y0 + y1)
 // - x0 y0 - x1 y1 (< 2 q^2); the operand sums stay below 2q < 2^160 and need no reduction.
-#ifndef PBC_F2_LAZY
-#define PBC_F2_LAZY 1
-#endif
 __device__ __noinline__ void f2_mul(F2* r, const F2* x, const F2* y) {
-  if (PBC_F2_LAZY && c_f.nice) {
+  if (c_f.nice) {
     Fq x0 = x->a, x1 = x->b, y0 = y->a, y1 = y->b, sx, sy;
     FqW t0, t1, t2, qq;
     fq_add_nr(sx, x0, x1);
@@ -112,16 +100,16 @@ __device__ __noinline__ void f2_mul(F2* r, const F2* x, const F2* y) {
   Fq t0, t1, t2, u;
   fq_add(t2, x->a, x->b);
   fq_add(u, y->a, y->b);
-  fq_mul_hot(t2, t2, u);
-  fq_mul_hot(t0, x->a, y->a);
-  fq_mul_hot(t1, x->b, y->b);
+  fq_mul(t2, t2, u);
+  fq_mul(t0, x->a, y->a);
+  fq_mul(t1, x->b, y->b);
   fq_sub(t2, t2, t0);
   fq_sub(t2, t2, t1);
   if (c_f.nice) {
     fq_sub(r->a, t0, t1);
   } else {
     fq_set(u, c_f.beta);
-    fq_mul_hot(t1, t1, u);
+    fq_mul(t1, t1, u);
     fq_add(r->a, t0, t1);
   }
   r->b = t2;
@@ -129,11 +117,11 @@ __device__ __noinline__ void f2_mul(F2* r, const F2* x, const F2* y) {
 // x0^2 + beta x1^2 + 2 x0 x1 s;  internal basis: (x0 + x1)(x0 - x1) + 2 x0 x1 i
 __device__ __noinline__ void f2_sqr(F2* r, const F2* x) {
   Fq t0, t1, t2, u;
-  fq_mul_hot(t2, x->a, x->b);
+  fq_mul(t2, x->a, x->b);
   if (c_f.nice) {
     fq_add(t0, x->a, x->b);
     fq_sub(t1, x->a, x->b);
-    fq_mul_hot(r->a, t0, t1);
+    fq_mul(r->a, t0, t1);
   } else {
     fq_sqr(t0, x->a);
     fq_sqr(t1, x->b);
@@ -363,7 +351,7 @@ __device__ __noinline__ void f12_mul_line(F12* v, const Fq* c, const F2* L3, con
   m4[1] = *L4;
   f2_mul_xi(m3[0], m3[1]);
   f2_mul_xi(m4[0], m4[1]);
-  if (PBC_F2_LAZY && c_f.nice) {
+  if (c_f.nice) {
     // every output coefficient is the sum of three products: accumulate them unreduced and reduce
     // once (5 q^2 < 2 q R: fq_redc2) -- 12 reductions per line instead of 36
 #pragma unroll
@@ -452,7 +440,7 @@ __device__ __noinline__ void f12_to_internal(F12& v) {
 // P: n1 x 40 bytes (stride1 = 0 shares one P: pairing_pp_*), Q: n x 80 bytes.
 // mv: [60][n] words, flag[n]: 1 = both inputs finite points on their curves.
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, (PBC_CC_MINBLOCKS * 128) / BLOCK)
+__global__ void __launch_bounds__(BLOCK, (kCCMinBlocks * 128) / BLOCK)
 k_f_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_t* __restrict__ mv,
            uint32_t* __restrict__ flag, size_t n, size_t stride1, const uint32_t* __restrict__ tab, size_t rows) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -503,7 +491,7 @@ k_f_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_
 // exponentiation is a homomorphism, so the k Miller values are multiplied here and exponentiated
 // once.  Any O input -> identity (include/pbc_pairing.h:161-168).
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_f_prod(const uint32_t* __restrict__ mv_in, const uint32_t* __restrict__ flag_in,
          uint32_t* __restrict__ mv_out, uint32_t* __restrict__ flag_out, size_t k, size_t n_out,
          size_t n_in) {
@@ -579,7 +567,7 @@ __device__ __noinline__ void f12_pow_u(F12& r, const F12& f) {
   F12 acc;
   acc = f;
   for (int j = (int)c_f.u_bits - 2; j >= 0; j--) {
-    if (PBC_CC_LOCKSTEP) __syncthreads();        // uniform loop: keep the block's warps in step
+    __syncthreads();        // uniform loop: keep the block's warps in step
     f12_cyc_sqr(&acc);
     if ((c_f.u_abs[j >> 5] >> (j & 31)) & 1u) f12_mul(&acc, &acc, &f);
   }
@@ -647,7 +635,7 @@ __device__ __noinline__ void f12_final_exp(F12& acc, F12& f) {
 // inversion, then the 472-bit power (q^4 - q^2 + 1)/r.  out: n x 240 bytes, coefficient order
 // x^0..x^5, each (re, im) (arith/poly.c:718-727, arith/fieldquadratic.c:323-329).
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, (PBC_CC_MINBLOCKS * 128) / BLOCK)
+__global__ void __launch_bounds__(BLOCK, (kCCMinBlocks * 128) / BLOCK)
 k_f_finalexp(const uint32_t* __restrict__ mv, const uint32_t* __restrict__ flag,
              uint8_t* __restrict__ out, size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;

@@ -27,12 +27,9 @@ namespace pbcb200 {
 // Slots per thread: 36 = 720 B, two 128-thread blocks (8 warps) per SM, about 210 registers per thread.
 // A 29-slot version (V = (X, Y, Z) and xi L3, xi L4 parked in the global scratch: three blocks = 12 warps
 // per SM, registers capped at 168) was slower: the cap spills inside the product routines.  These kernels want registers more than they want warps.
-// PBC_FS_LOCKSTEP = 1: block-wide barrier at the top of every Miller iteration and of every step of the
-// powers by u, so that the warps of a block fetch the same routines (without it k_f_finalexp_s waits on
-// instruction fetch).  Every thread of a block then has to run the loops.
-#ifndef PBC_FS_LOCKSTEP
-#define PBC_FS_LOCKSTEP 1
-#endif
+// A block-wide barrier at the top of every Miller iteration and of every step of the powers by u keeps the
+// warps of a block fetching the same routines (without it k_f_finalexp_s waits on instruction fetch).  Every
+// thread of a block then has to run the loops.
 constexpr int kFSlots = 36;
 enum FSlotMap {
   fsV = 0,                             // 12: Miller value (coefficient j at 2 * f12_pos(j))
@@ -45,46 +42,23 @@ enum FSlotMap {
 enum FGlobalMap { fgQx = 0, fgQy = 2, fgPx = 4, fgPy = 5 };
 constexpr int kFGWords = 6 * kNS;
 
-// ---- register-level pieces (fqw_mul, fqw_redc2: fq_small.cuh) ----
-// r = a b (Montgomery): interleaved column-wise product, or wide product + two-product reduction
-__device__ __forceinline__ void fq_mul_sel(Fq& r, const Fq& a, const Fq& b) {
-  if (PBC_FQ_ACC) fq_mul_os(r, a, b);
-  else if (PBC_FQW_REDC_SPLIT) { FqW t; fqw_mul(t, a, b); fqw_redc_split(r, t); }
-  else mont_mul_ps<kNS, false>(r.v, a.v, b.v);
-}
-// r = a^2.  PBC_FS_SQR_OS: the full 25-product row schedule (fewer instructions); else the 15 + 25 product
-// column-wise squarer.
-#ifndef PBC_FS_SQR_OS
-#define PBC_FS_SQR_OS PBC_FQ_ACC
-#endif
-__device__ __forceinline__ void fq_sqr_sel(Fq& r, const Fq& a) {
-  if (PBC_FS_SQR_OS) fq_mul_os(r, a, a); else mont_sqr_ps<kNS, false>(r.v, a.v);
-}
+// ---- register-level pieces (fq_small.cuh) ----
+// Products and squares alike are fq_mul_os: the full 25-product row schedule takes fewer instructions than
+// the 15 + 25 product column-wise squarer.
 
-// ---- F_q^2 products on three unmerged sums (fq_small.cuh, PBC_FQ_ACC) ----
+// ---- F_q^2 products on three unmerged sums (FqAcc, fq_small.cuh) ----
 //   A = sum x0 y0,  B = sum x1 y1,  C = sum (x0 + x1)(y0 + y1);   re = A - B,  im = C - A - B.
 // Bounds: operands canonical, so a term adds less than q^2 to A and B and less than 4 q^2 to C; three terms
 // keep C below 12 q^2 < 2^320 (c_f.slots_ok).
 struct F2Acc { FqAcc A, B, C; };
-// PBC_F2A_FENCE = 1: a warp-level barrier between the products of a term.  It computes nothing; it keeps ptxas from
-// interleaving the carry runs of more products than there are carry predicates (seven): in f12's line product it
-// had a dozen runs in flight and spent 12 % of the routine saving and restoring predicates (LOP3 / P2R).
-#ifndef PBC_F2A_FENCE
-#define PBC_F2A_FENCE 0
-#endif
-__device__ __forceinline__ void f2a_fence() {
-#if PBC_F2A_FENCE
-  __syncwarp();
-#endif
-}
 // TERM 0: the first term (starts the sums), 1: the second (first carry counts), 2: any later one
 template <int TERM>
 __device__ __forceinline__ void f2a_term(F2Acc& g, const Fq& x0, const Fq& x1, const Fq& y0, const Fq& y1) {
   Fq sx, sy;
   fq_add_nr(sx, x0, x1);
   fq_add_nr(sy, y0, y1);
-  if (TERM == 0) { fqa_mul(g.A, x0, y0); f2a_fence(); fqa_mul(g.B, x1, y1); f2a_fence(); fqa_mul(g.C, sx, sy); f2a_fence(); }
-  else { fqa_mac<TERM == 1>(g.A, x0, y0); f2a_fence(); fqa_mac<TERM == 1>(g.B, x1, y1); f2a_fence(); fqa_mac<TERM == 1>(g.C, sx, sy); f2a_fence(); }
+  if (TERM == 0) { fqa_mul(g.A, x0, y0); fqa_mul(g.B, x1, y1); fqa_mul(g.C, sx, sy); }
+  else { fqa_mac<TERM == 1>(g.A, x0, y0); fqa_mac<TERM == 1>(g.B, x1, y1); fqa_mac<TERM == 1>(g.C, sx, sy); }
 }
 // (r0, r1) = (re, im) reduced.  offs: a multiple of q^2 (double width) not below B, HASK: more than one term.
 template <bool HASK>
@@ -103,23 +77,6 @@ __device__ __forceinline__ void f2a_finish(Fq& r0, Fq& r1, const F2Acc& g, const
   fqw_redc_os<true>(r1, c);
 }
 
-// (re, im) += x y for F_q^2 operands in the internal basis (i^2 = -1), double width, unreduced:
-//   re += x0 y0 - x1 y1,  im += (x0 + x1)(y0 + y1) - x0 y0 - x1 y1.
-// The caller starts re at (number of terms) * q^2 so that it never goes negative.
-__device__ __forceinline__ void f2w_mac(FqW& re, FqW& im, const Fq& x0, const Fq& x1, const Fq& y0, const Fq& y1) {
-  Fq sx, sy;
-  FqW t;
-  fq_add_nr(sx, x0, x1);
-  fq_add_nr(sy, y0, y1);
-  fqw_mul(t, sx, sy);
-  fqw_add(im, im, t);
-  fqw_mul(t, x0, y0);
-  fqw_add(re, re, t);
-  fqw_sub(im, im, t);
-  fqw_mul(t, x1, y1);
-  fqw_sub(re, re, t);
-  fqw_sub(im, im, t);
-}
 // (x0 + x1 i) <- xi' (x0 + x1 i), xi' = a + b i with small a, b (see f2_mul_xi)
 __device__ __forceinline__ void f2r_mul_xi(Fq& x0, Fq& x1) {
   const uint32_t a = c_f.xi_a, b = c_f.xi_b, m = a | b;
@@ -139,8 +96,8 @@ __device__ __forceinline__ void f2r_sqr(Fq& o0, Fq& o1, const Fq& x0, const Fq& 
   Fq s, t;
   fq_add_nr(s, x0, x1);                    // below 2q < 2^160: fine as a multiplier operand
   fq_sub(t, x0, x1);
-  fq_mul_sel(s, s, t);
-  fq_mul_sel(t, x0, x1);
+  fq_mul_os(s, s, t);
+  fq_mul_os(t, x0, x1);
   fq_dbl(o1, t);
   o0 = s;
 }
@@ -169,9 +126,6 @@ __device__ __forceinline__ void gs_combine(Fq& c, const Fq& r) {
 // ---- the slot machine ----
 template <int BLOCK>
 struct FS {
-  // PBC_FS_LOCKSTEP >= 2: a block-wide barrier before every big routine as well (F_q^6 products, line product), not only
-  // at the top of an iteration
-  static __device__ __forceinline__ void step_barrier() { if (PBC_FS_LOCKSTEP >= 2) __syncthreads(); }
   static __device__ __forceinline__ uint32_t* base() { return reinterpret_cast<uint32_t*>(pbc_smem) + threadIdx.x; }
   static __device__ __forceinline__ void ld(Fq& r, int s) {
     const uint32_t* b = base() + s * (kNS * BLOCK);
@@ -187,75 +141,51 @@ struct FS {
   static __device__ __noinline__ void qmul(int d, int a, int b) {
     Fq x, y;
     ld(x, a); ld(y, b);
-    fq_mul_sel(x, x, y);
+    fq_mul_os(x, x, y);
     st(d, x);
   }
   static __device__ __noinline__ void qsqr(int d, int a) {
     Fq x;
     ld(x, a);
-    fq_sqr_sel(x, x);
+    fq_mul_os(x, x, x);
     st(d, x);
   }
   // two / three independent products in ONE call, every operand read before any result is stored (so the
   // results may overwrite operands of the other products).  A lone F_q product is one serial carry chain;
   // the point arithmetic of a Miller step has them in independent pairs and triples, and two warps per
   // scheduler do not hide a chain's latency.
-  // PBC_FS_ONE_QMUL = 1: the grouped calls below run their products one after the other through qmul / qsqr (one copy
-  // of the multiplier in the loop body instead of nine: 25 KB less code to fetch per iteration; an A/B experiment)
-#ifndef PBC_FS_ONE_QMUL
-#define PBC_FS_ONE_QMUL 0
-#endif
-#if PBC_FS_ONE_QMUL
-  static __device__ __forceinline__ void qmul2(int d0, int a0, int b0, int d1, int a1, int b1) {
-    Fq x0, x1;                                    // every operand is read before any result is stored
-    ld(x0, a1); ld(x1, b1);
-    qmul(d0, a0, b0);
-    qmul_r(d1, x0, x1);
-  }
-  static __device__ __noinline__ void qmul_r(int d, Fq x, Fq y) { fq_mul_sel(x, x, y); st(d, x); }
-  static __device__ __forceinline__ void qmul3(int d0, int a0, int b0, int d1, int a1, int b1, int d2, int a2, int b2) {
-    Fq x1, y1, x2, y2;
-    ld(x1, a1); ld(y1, b1); ld(x2, a2); ld(y2, b2);
-    qmul(d0, a0, b0);
-    qmul_r(d1, x1, y1);
-    qmul_r(d2, x2, y2);
-  }
-  static __device__ __forceinline__ void qsqr3(int d0, int a0, int d1, int a1, int d2, int a2) { qmul3(d0, a0, a0, d1, a1, a1, d2, a2, a2); }
-  static __device__ __forceinline__ void qmul1sqr2(int d0, int a0, int b0, int d1, int a1, int d2, int a2) { qmul3(d0, a0, b0, d1, a1, a1, d2, a2, a2); }
-#else
   static __device__ __noinline__ void qmul2(int d0, int a0, int b0, int d1, int a1, int b1) {
     Fq x0, y0, x1, y1;
     ld(x0, a0); ld(y0, b0); ld(x1, a1); ld(y1, b1);
-    fq_mul_sel(x0, x0, y0);
-    fq_mul_sel(x1, x1, y1);
+    fq_mul_os(x0, x0, y0);
+    fq_mul_os(x1, x1, y1);
     st(d0, x0); st(d1, x1);
   }
   static __device__ __noinline__ void qmul3(int d0, int a0, int b0, int d1, int a1, int b1, int d2, int a2, int b2) {
     Fq x0, y0, x1, y1, x2, y2;
     ld(x0, a0); ld(y0, b0); ld(x1, a1); ld(y1, b1); ld(x2, a2); ld(y2, b2);
-    fq_mul_sel(x0, x0, y0);
-    fq_mul_sel(x1, x1, y1);
-    fq_mul_sel(x2, x2, y2);
+    fq_mul_os(x0, x0, y0);
+    fq_mul_os(x1, x1, y1);
+    fq_mul_os(x2, x2, y2);
     st(d0, x0); st(d1, x1); st(d2, x2);
   }
   static __device__ __noinline__ void qsqr3(int d0, int a0, int d1, int a1, int d2, int a2) {
     Fq x0, x1, x2;
     ld(x0, a0); ld(x1, a1); ld(x2, a2);
-    fq_sqr_sel(x0, x0);
-    fq_sqr_sel(x1, x1);
-    fq_sqr_sel(x2, x2);
+    fq_mul_os(x0, x0, x0);
+    fq_mul_os(x1, x1, x1);
+    fq_mul_os(x2, x2, x2);
     st(d0, x0); st(d1, x1); st(d2, x2);
   }
   // d0 = a0 b0, d1 = a1^2, d2 = a2^2
   static __device__ __noinline__ void qmul1sqr2(int d0, int a0, int b0, int d1, int a1, int d2, int a2) {
     Fq x0, y0, x1, x2;
     ld(x0, a0); ld(y0, b0); ld(x1, a1); ld(x2, a2);
-    fq_mul_sel(x0, x0, y0);
-    fq_sqr_sel(x1, x1);
-    fq_sqr_sel(x2, x2);
+    fq_mul_os(x0, x0, y0);
+    fq_mul_os(x1, x1, x1);
+    fq_mul_os(x2, x2, x2);
     st(d0, x0); st(d1, x1); st(d2, x2);
   }
-#endif
   static __device__ __noinline__ void qadd(int d, int a, int b) { Fq x, y; ld(x, a); ld(y, b); fq_add(x, x, y); st(d, x); }
   static __device__ __noinline__ void qsub(int d, int a, int b) { Fq x, y; ld(x, a); ld(y, b); fq_sub(x, x, y); st(d, x); }
   static __device__ __noinline__ void qdbl(int d, int a, int k = 1) {
@@ -287,8 +217,8 @@ struct FS {
 #pragma unroll
     for (int k = 0; k < kNS; k++) { y0.v[k] = g[((size_t)e * kNS + k) * n]; y1.v[k] = g[((size_t)(e + 1) * kNS + k) * n]; }
     ld(x, a);
-    fq_mul_sel(y0, y0, x);
-    fq_mul_sel(y1, y1, x);
+    fq_mul_os(y0, y0, x);
+    fq_mul_os(y1, y1, x);
     st(d, y0); st(d + 1, y1);
   }
   // ---- F_q^2 (two consecutive slots) ----
@@ -320,8 +250,8 @@ struct FS {
     ld(x0, a); ld(x1, a + 1);
     fq_add_nr(s, x0, x1);                  // below 2q < 2^160: fine as a multiplier operand
     fq_sub(t, x0, x1);
-    fq_mul_sel(s, s, t);
-    fq_mul_sel(t, x0, x1);
+    fq_mul_os(s, s, t);
+    fq_mul_os(t, x0, x1);
     fq_dbl(t, t);
     st(d, s); st(d + 1, t);
   }
@@ -344,18 +274,9 @@ struct FS {
     ld(x0, a); ld(x1, a + 1);
     if (conj) fq_neg(x1, x1);
     fq_set(y0, c[0]); fq_set(y1, c[1]);
-#if PBC_FQ_ACC
     F2Acc g;
     f2a_term<0>(g, x0, x1, y0, y1);
     f2a_finish<false>(x0, x1, g, c_f.qsqm[0]);
-#else
-    FqW re, im;
-#pragma unroll
-    for (int w = 0; w < 2 * kNS; w++) { re.v[w] = c_f.qsqm[0][w]; im.v[w] = 0; }
-    f2w_mac(re, im, x0, x1, y0, y1);
-    fqw_reduce(x0, re);
-    fqw_reduce(x1, im);
-#endif
     st(d, x0); st(d + 1, x1);
   }
 
@@ -365,7 +286,6 @@ struct FS {
   // reduction per F_q.
   // xs: four scratch slots (they receive xi b_1 and xi b_2), apart from d, a, b.
   static __device__ __noinline__ void f6mul(int d, int a, int b, int xs) {
-#if PBC_FQ_ACC
     // The three terms of a coefficient are written out: sums carried around a loop cost a register move per
     // accumulator pair and iteration.  The
     // wrapped operands xi b_1, xi b_2 are made once, so a term only selects its slot.
@@ -373,7 +293,6 @@ struct FS {
     f2mulxi(xs + 2, b + 4);
 #pragma unroll 1
     for (int k = 0; k < 3; k++) {
-      if (PBC_FS_LOCKSTEP >= 3) __syncthreads();
       F2Acc g;
       Fq x0, x1, y0, y1;
       ld(x0, a); ld(x1, a + 1); ld(y0, b + 2 * k); ld(y1, b + 2 * k + 1);      // a_0 b_k
@@ -387,30 +306,6 @@ struct FS {
       f2a_finish<true>(x0, x1, g, c_f.qsqm[2]);
       st(d + 2 * k, x0); st(d + 2 * k + 1, x1);
     }
-#else
-    (void)xs;
-#pragma unroll 1
-    for (int k = 0; k < 3; k++) {
-      FqW re, im;
-#pragma unroll
-      for (int w = 0; w < 2 * kNS; w++) { re.v[w] = c_f.qsqm[2][w]; im.v[w] = 0; }
-#pragma unroll 1
-      for (int i = 0; i < 3; i++) {
-        int j = k - i;
-        const bool wrap = j < 0;
-        if (wrap) j += 3;
-        Fq x0, x1, y0, y1;
-        ld(y0, b + 2 * j); ld(y1, b + 2 * j + 1);
-        if (wrap) f2r_mul_xi(y0, y1);
-        ld(x0, a + 2 * i); ld(x1, a + 2 * i + 1);
-        f2w_mac(re, im, x0, x1, y0, y1);
-      }
-      Fq r0, r1;
-      fqw_reduce(r0, re);
-      fqw_reduce(r1, im);
-      st(d + 2 * k, r0); st(d + 2 * k + 1, r1);
-    }
-#endif
   }
   // o = v * (c + L3 x^3 + L4 x^4)   (f12_mul_line): o and v are 12-slot F_q^12 areas, distinct.
   //   o_k = c v_k + m3 v_(k-3) + m4 v_(k-4), indices below zero wrap with xi (slots fsXL3 / fsXL4)
@@ -418,8 +313,6 @@ struct FS {
 #pragma unroll 1
     for (int k = 0; k < 6; k++) {
       const int i3 = k >= 3 ? k - 3 : k + 3, i4 = k >= 4 ? k - 4 : k + 2;
-      if (PBC_FS_LOCKSTEP >= 3) __syncthreads();
-#if PBC_FQ_ACC
       // re = A - B + c y0,  im = C - A - B + c y1:  c y0 joins A and c (y0 + y1) joins C
       F2Acc g;
       Fq x0, x1, y0, y1;
@@ -434,43 +327,17 @@ struct FS {
       ld(y0, v + 2 * f12_pos(k)); ld(y1, v + 2 * f12_pos(k) + 1);
       fq_add_nr(x1, y0, y1);
       fqa_mac<false>(g.A, x0, y0);
-      f2a_fence();
       fqa_mac<false>(g.C, x0, x1);
-      f2a_fence();
       f2a_finish<true>(x0, x1, g, c_f.qsqm[1]);
       st(o + 2 * f12_pos(k), x0); st(o + 2 * f12_pos(k) + 1, x1);
-#else
-      FqW re, im, t;
-#pragma unroll
-      for (int w = 0; w < 2 * kNS; w++) { re.v[w] = c_f.qsqm[1][w]; im.v[w] = 0; }
-      Fq x0, x1, y0, y1;
-      const int m3 = k >= 3 ? fsL3 : fsXL3, m4 = k >= 4 ? fsL4 : fsXL4;
-      ld(x0, m3); ld(x1, m3 + 1);
-      ld(y0, v + 2 * f12_pos(i3)); ld(y1, v + 2 * f12_pos(i3) + 1);
-      f2w_mac(re, im, x0, x1, y0, y1);
-      ld(x0, m4); ld(x1, m4 + 1);
-      ld(y0, v + 2 * f12_pos(i4)); ld(y1, v + 2 * f12_pos(i4) + 1);
-      f2w_mac(re, im, x0, x1, y0, y1);
-      ld(x0, fsC);
-      ld(y0, v + 2 * f12_pos(k)); ld(y1, v + 2 * f12_pos(k) + 1);
-      fqw_mul(t, x0, y0);
-      fqw_add(re, re, t);
-      fqw_mul(t, x0, y1);
-      fqw_add(im, im, t);
-      fqw_reduce(x0, re);
-      fqw_reduce(x1, im);
-      st(o + 2 * f12_pos(k), x0); st(o + 2 * f12_pos(k) + 1, x1);
-#endif
     }
   }
   // v <- v^2 in place with the 12-slot scratch t (f12_sqr: complex squaring over F_q^6).
   //   A = v[0..5], B = v[6..11];  t0 = A B;  t1 = (A + B)(A + y B);  A' = t1 - t0 - y t0,  B' = 2 t0
   static __device__ __forceinline__ void f12sqr(int v, int t, int xs) {
-    step_barrier();
     f6mul(t, v, v + 6, xs);                                    // t0
     f2add(t + 6, v, v + 6); f2add(t + 8, v + 2, v + 8); f2add(t + 10, v + 4, v + 10);        // A + B
     f2addxi(v, v, v + 10); f2add(v + 2, v + 2, v + 6); f2add(v + 4, v + 4, v + 8);           // A + y B, in place
-    step_barrier();
     f6mul(v + 6, t + 6, v, xs);                                // t1 over B (B is dead)
     f2sub(v, v + 6, t); f2subxi(v, v, t + 4);                  // A'0 = t1_0 - t0_0 - xi t0_2
     f2sub(v + 2, v + 8, t + 2); f2sub(v + 2, v + 2, t);        // A'1 = t1_1 - t0_1 - t0_0
@@ -480,13 +347,10 @@ struct FS {
   // p <- p q with the 12-slot scratch t (f12_mul: Karatsuba over F_q^6); q is left as it was.
   //   p = A + B x, q = C + D x:  t0 = A C, t1 = B D, t2 = (A + B)(C + D);  lo = t0 + y t1, hi = t2 - t0 - t1
   static __device__ __forceinline__ void f12mul(int p, int q, int t, int xs) {
-    step_barrier();
     f6mul(t, p, q, xs);                                        // t0
-    step_barrier();
     f6mul(t + 6, p + 6, q + 6, xs);                            // t1
     f2add(p, p, p + 6); f2add(p + 2, p + 2, p + 8); f2add(p + 4, p + 4, p + 10);     // A + B over A
     f2add(q, q, q + 6); f2add(q + 2, q + 2, q + 8); f2add(q + 4, q + 4, q + 10);     // C + D over C
-    step_barrier();
     f6mul(p + 6, p, q, xs);                                    // t2 over B
     f2sub(q, q, q + 6); f2sub(q + 2, q + 2, q + 8); f2sub(q + 4, q + 4, q + 10);     // C back
     f2sub(p + 6, p + 6, t); f2sub(p + 6, p + 6, t + 6);
@@ -514,12 +378,9 @@ struct FS {
   // History: 28 calls of F_q^2 routines per squaring ran at 0.3 of the multiplier peak (5.5 instructions per
   // product); two fused routines working in registers (cyc_pair_a, cyc_pair_bc: the three F_q^4 squarings written out,
   // 2 200 instructions executed once per squaring) left the warps waiting for instructions
-  // in k_f_finalexp_s.  PBC_FS_CYC_ONE = 1: ONE out-of-line F_q^4 squaring
+  // in k_f_finalexp_s.  Now ONE out-of-line F_q^4 squaring
   // with the recombination, called three times (B's square waits in the four scratch slots e while C -- which reads
   // what B's results overwrite -- is done).
-#ifndef PBC_FS_CYC_ONE
-#define PBC_FS_CYC_ONE 1
-#endif
   // (r0, r1) = (a + b s)^2 for the F_q^2 at slots a, b.  raw: tm <- r0, tp <- r1;  else tm <- 3 r0 - 2 tm and
   // tp <- 3 r1' + 2 tp with r1' = xi r1 when xi is set.
   static __device__ __noinline__ void f4sqr_gs(int a, int b, int tm, int tp, bool raw, bool xi) {
@@ -535,41 +396,13 @@ struct FS {
     }
     st(tm, r00); st(tm + 1, r01); st(tp, r10); st(tp + 1, r11);
   }
-  static __device__ __noinline__ void cyc_pair_a(int v) {
-    Fq a0, a1, b0, b1, r00, r01, r10, r11;
-    ld(a0, v); ld(a1, v + 1); ld(b0, v + 8); ld(b1, v + 9);
-    f4r_sqr(r00, r01, r10, r11, a0, a1, b0, b1);
-    gs_combine<false>(a0, r00); gs_combine<false>(a1, r01);
-    gs_combine<true>(b0, r10); gs_combine<true>(b1, r11);
-    st(v, a0); st(v + 1, a1); st(v + 8, b0); st(v + 9, b1);
-  }
-  static __device__ __noinline__ void cyc_pair_bc(int v) {
-    Fq c10, c11, c40, c41, c20, c21, c50, c51;
-    Fq B00, B01, B10, B11, C00, C01, C10, C11;
-    ld(c10, v + 6); ld(c11, v + 7); ld(c40, v + 4); ld(c41, v + 5);
-    f4r_sqr(B00, B01, B10, B11, c10, c11, c40, c41);
-    ld(c20, v + 2); ld(c21, v + 3); ld(c50, v + 10); ld(c51, v + 11);
-    f4r_sqr(C00, C01, C10, C11, c20, c21, c50, c51);
-    gs_combine<false>(c20, B00); gs_combine<false>(c21, B01);
-    gs_combine<true>(c50, B10); gs_combine<true>(c51, B11);
-    f2r_mul_xi(C10, C11);
-    gs_combine<true>(c10, C10); gs_combine<true>(c11, C11);
-    gs_combine<false>(c40, C00); gs_combine<false>(c41, C01);
-    st(v + 2, c20); st(v + 3, c21); st(v + 10, c50); st(v + 11, c51);
-    st(v + 6, c10); st(v + 7, c11); st(v + 4, c40); st(v + 5, c41);
-  }
   // e: four scratch slots
   static __device__ __forceinline__ void f12cycsqr(int v, int, int e) {
-    if (PBC_FS_CYC_ONE) {
-      f4sqr_gs(v + 6, v + 4, e, e + 2, true, false);            // B -> scratch
-      f4sqr_gs(v, v + 8, v, v + 8, false, false);               // A
-      f4sqr_gs(v + 2, v + 10, v + 4, v + 6, false, true);       // C (reads c2, c5; writes c4, c1)
-      f2gs<false>(v + 2, e, v + 2);                             // c2' = 3 B0 - 2 c2
-      f2gs<true>(v + 10, e + 2, v + 10);                        // c5' = 3 B1 + 2 c5
-    } else {
-      cyc_pair_a(v);
-      cyc_pair_bc(v);
-    }
+    f4sqr_gs(v + 6, v + 4, e, e + 2, true, false);            // B -> scratch
+    f4sqr_gs(v, v + 8, v, v + 8, false, false);               // A
+    f4sqr_gs(v + 2, v + 10, v + 4, v + 6, false, true);       // C (reads c2, c5; writes c4, c1)
+    f2gs<false>(v + 2, e, v + 2);                             // c2' = 3 B0 - 2 c2
+    f2gs<true>(v + 10, e + 2, v + 10);                        // c5' = 3 B1 + 2 c5
   }
   // v <- v^(q^k), k = 1, 2, 3 (f12_frob)
   static __device__ __noinline__ void f12frob(int v, int k) {
@@ -602,7 +435,7 @@ struct FS {
   static __device__ __noinline__ void f12powu(int r0, int r1, int t, int e) {
     f12copy(r0, r1);
     for (int j = (int)c_f.u_bits - 2; j >= 0; j--) {
-      if (PBC_FS_LOCKSTEP) __syncthreads();
+      __syncthreads();
       f12cycsqr(r0, t, e);
       if ((c_f.u_abs[j >> 5] >> (j & 31)) & 1u) f12mul(r0, r1, t, e);
     }
@@ -612,22 +445,14 @@ struct FS {
 
 // Same interface as k_f_miller plus gq: [6 * kNS][n] words of scratch (Qx, Qy untwisted and scaled, P;
 // Montgomery form, internal basis).
-// PBC_FS_MILLER_MAXREG: register cap of the Miller kernel (for block sizes where the default would cost a
-// resident block); not defined = no cap
-#ifdef PBC_FS_MILLER_MAXREG
-#define PBC_FS_MILLER_BOUNDS __maxnreg__(PBC_FS_MILLER_MAXREG)
-#else
-#define PBC_FS_MILLER_BOUNDS __launch_bounds__(BLOCK)
-#endif
 template <int BLOCK>
-__global__ void PBC_FS_MILLER_BOUNDS
+__global__ void __launch_bounds__(BLOCK)
 k_f_miller_s(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_t* __restrict__ mv,
              uint32_t* __restrict__ flag, uint32_t* __restrict__ gq, size_t n, size_t stride1,
              const uint32_t* __restrict__ tab, size_t rows) {
   using S = FS<BLOCK>;
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   const bool live = idx < n;               // padding threads of the last block run too (block-wide barriers below)
-  if (!PBC_FS_LOCKSTEP && !live) return;
   if (!live) idx = 0;
   bool ok;
   {
@@ -671,13 +496,9 @@ k_f_miller_s(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint3
   const uint32_t* g = gq + idx;
   int V = fsV, T = fsT;
   size_t row = 0;
-#if PBC_CC_NAF
   int m = (int)c_ccnaf.len - 2;
-#else
-  int m = (int)c_cc.rbits - 2;
-#endif
   for (;;) {
-    if (PBC_FS_LOCKSTEP) __syncthreads();
+    __syncthreads();
     if (tab) {
       // ---- fixed first argument: (a, b, c) of the next line from the table ----
       S::qldc(T + 4, tab + (3 * row + 0) * kNS); S::f2scale_g(fsL4, g, 0, n, T + 4);
@@ -707,17 +528,11 @@ k_f_miller_s(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint3
       S::qsub(T + 5, T + 5, fsX); S::qmul(fsY, T + 1, T + 5); S::qsub(fsY, fsY, T + 2);   // Y'
     }
     }
-    S::step_barrier();
     S::line_mul(T, V);
     { int s = V; V = T; T = s; }
     if (m == 0) break;
-#if PBC_CC_NAF
     if ((c_ccnaf.nz[m >> 5] >> (m & 31)) & 1u) {
       const bool minus = (c_ccnaf.neg[m >> 5] >> (m & 31)) & 1u;
-#else
-    if ((c_cc.r[m >> 5] >> (m & 31)) & 1u) {
-      const bool minus = false;
-#endif
       if (tab) {
         S::qldc(T + 4, tab + (3 * row + 0) * kNS); S::f2scale_g(fsL4, g, 0, n, T + 4);
         S::qldc(T + 4, tab + (3 * row + 1) * kNS); S::f2scale_g(fsL3, g, 2, n, T + 4);
@@ -725,7 +540,6 @@ k_f_miller_s(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint3
         S::f2mulxi(fsXL3, fsL3); S::f2mulxi(fsXL4, fsL4);
         row++;
       } else {
-      (void)minus;
       // ---- chord through V and +-P (a = Y - yS Z^3, b = (xP Z^2 - X) Z, c = yS Z X - xP Y), V <- V +- P ----
       // (14 products in six calls of independent pairs / triples)
       S::qldg(T + 6, g, 4, n, false);                    // xP
@@ -748,7 +562,6 @@ k_f_miller_s(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint3
       S::qmul2(T, T, T + 3, T + 1, T + 1, fsY);                          // R (X H^2 - X3), H^3 Y
       S::qsub(fsY, T, T + 1);                                            // Y3
       }
-      S::step_barrier();
       S::line_mul(T, V);
       { int s = V; V = T; T = s; }
     }
@@ -787,7 +600,6 @@ k_f_finalexp_s(uint32_t* __restrict__ mv, const uint32_t* __restrict__ flag, uin
   enum { R0 = 0, R1 = 12, T = 24, E = 36 };
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
   const bool live = idx < n;               // padding threads run the powers by u too (block-wide barriers inside)
-  if (!PBC_FS_LOCKSTEP && !live) return;
   if (!live) idx = 0;
   const bool ok = flag[idx] != 0;
   uint32_t* g0 = mv + idx;                                     // f

@@ -99,51 +99,9 @@ __device__ __noinline__ void f5_mul(F5* r, const F5* x, const F5* y) {
   }
   *r = o;
 }
-// Two things that did not pay here: a dedicated squaring with the ten cross products doubled (15 + 20
-// products but more code) and the lock-step barrier in the Lucas ladder; both stay behind switches.
-#ifndef PBC_G_SQR
-#define PBC_G_SQR 0
-#endif
-#ifndef PBC_G_FINAL_LOCKSTEP
-#define PBC_G_FINAL_LOCKSTEP 0
-#endif
-// x^2: the 10 cross products once and doubled, the 5 squares, then the same folding (15 + 20 products)
-#if PBC_G_SQR
-__device__ __noinline__ void f5_sqr(F5* r, const F5* x) {
-  FqW d[9], t;
-  Fq hi[4], k;
-  F5 o;
-#pragma unroll 1
-  for (int s = 0; s < 9; s++) {
-    bool first = true;
-#pragma unroll 1
-    for (int i = (s < 5 ? 0 : s - 4); 2 * i < s; i++) {          // i < s - i
-      t = fq_mulw_call(x->c[i], x->c[s - i]);
-      if (first) { d[s] = t; first = false; } else fqw_add(d[s], d[s], t);
-    }
-    if (!first) fqw_add(d[s], d[s], d[s]);
-    if ((s & 1) == 0) {
-      t = fq_mulw_call(x->c[s / 2], x->c[s / 2]);
-      if (first) { d[s] = t; first = false; } else fqw_add(d[s], d[s], t);
-    }
-  }
-#pragma unroll 1
-  for (int s = 0; s < 4; s++) hi[s] = fq_redc_call(d[5 + s]);
-#pragma unroll 1
-  for (int i = 0; i < 5; i++) {
-#pragma unroll 1
-    for (int s = 0; s < 4; s++) {
-      fq_set(k, c_g.xpwr[s][i]);
-      t = fq_mulw_call(hi[s], k);
-      fqw_add(d[i], d[i], t);
-    }
-    o.c[i] = fq_redc_call(d[i]);
-  }
-  *r = o;
-}
-#else
+// x^2 = x x: a dedicated squaring with the ten cross products doubled (15 + 20 products but more code) did not
+// pay here (DESIGN.md §3.8)
 __device__ __forceinline__ void f5_sqr(F5* r, const F5* x) { f5_mul(r, x, x); }
-#endif
 
 // (sum c_i x^i)^q = c0 + sum_{i >= 1} c_i x^(iq)   (ecc/g_param.c:483-493)
 __device__ __noinline__ void f5_frob(F5* r, const F5* x) {
@@ -277,7 +235,7 @@ __device__ __forceinline__ void f10_to_wire(uint8_t* p, const F10& v) {
 
 // P: 38 bytes each (stride1 = 0 shares one P), Q: n x 190 bytes (x: 5 coefficients, y: 5).
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, (PBC_CC_MINBLOCKS * 128) / BLOCK)
+__global__ void __launch_bounds__(BLOCK, (kCCMinBlocks * 128) / BLOCK)
 k_g_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_t* __restrict__ mv,
            uint32_t* __restrict__ flag, size_t n, size_t stride1, const uint32_t* __restrict__ tab, size_t rows) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
@@ -327,7 +285,7 @@ k_g_miller(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint32_
 
 // generic_prod_pairings (ecc/pairing.c:35-46): product of the k Miller values, one final power
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, PBC_CC_MINBLOCKS)
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
 k_g_prod(const uint32_t* __restrict__ mv_in, const uint32_t* __restrict__ flag_in,
          uint32_t* __restrict__ mv_out, uint32_t* __restrict__ flag_out, size_t k, size_t n_out,
          size_t n_in) {
@@ -367,7 +325,6 @@ __device__ __noinline__ void f10_final_exp(F5& out0, F5& out1, F10& f) {
   v0 = two;
   v1 = t1;
   for (int j = (int)c_g.phibits - 1; j >= 0; j--) {
-    if (PBC_CC_LOCKSTEP && PBC_G_FINAL_LOCKSTEP) __syncthreads();   // uniform ladder: keep the block's warps in step
     bool bit = j > 0 && ((c_g.phikonr[j >> 5] >> (j & 31)) & 1u);   // last step: clear branch
     f5_mul(&tmp, &v0, &v1);
     f5_sub(tmp, tmp, t1);
@@ -396,16 +353,16 @@ __device__ __noinline__ void f10_final_exp(F5& out0, F5& out1, F10& f) {
 
 // out: n x 190 bytes: real half (5 coefficients) then imaginary half
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, (PBC_CC_MINBLOCKS * 128) / BLOCK)
+__global__ void __launch_bounds__(BLOCK, (kCCMinBlocks * 128) / BLOCK)
 k_g_finalexp(const uint32_t* __restrict__ mv, const uint32_t* __restrict__ flag,
              uint8_t* __restrict__ out, size_t n) {
   size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
-  const bool live = idx < n;             // the ladder may hold block-wide barriers (PBC_G_FINAL_LOCKSTEP): no early exit
+  const bool live = idx < n;             // padding threads run on entry 0 and store nothing
   if (!live) idx = 0;
   F10 f;
   F5 out0, out1;
   const bool ok = flag[idx] != 0;
-  // every thread runs the ladder (block-wide barriers inside); flagged-off entries power 1
+  // flagged-off entries power 1
   f10_ld_global(f, mv, n, idx);
   if (!ok) f10_one(f);
   f10_final_exp(out0, out1, f);

@@ -4,7 +4,9 @@
 // memory slots, Montgomery limbs); here the same templates run against a big-integer policy class,
 // following k_a1_miller / k_a1_finalexp step for step, so the formulas (Jacobian doubling with the
 // tangent, chord + mixed addition, Lucas final exponentiation) are pinned to reference fixtures
-// without a GPU.  Argument "pp": go through the fixed-argument table programs instead; "5t": the five-temporary Miller programs; "naf" / "5t-naf": the signed-digit scan of n.  stdin: p n l count, then count lines "Px Py Qx Qy" (decimal); stdout: "Re Im" (hex).
+// without a GPU.  The Miller loop runs the five-temporary programs; argument "5t": on the bits of n, "5t-naf": on its
+// signed digits (as k_a1_miller), "pp": on the bits of n, then the fixed-argument table programs must give the same
+// pairing.  stdin: p n l count, then count lines "Px Py Qx Qy" (decimal); stdout: "Re Im" (hex).
 #include <stdio.h>
 #include <iostream>
 #include <string>
@@ -66,8 +68,7 @@ int main(int argc, char** argv) {
   using namespace pbcb200;
   const bool pp_mode = argc > 1 && std::string(argv[1]) == "pp";
   const std::string mode = argc > 1 ? argv[1] : "";
-  const bool five = mode == "5t" || mode == "5t-naf";           // the five-temporary programs
-  const bool naf = mode == "naf" || mode == "5t-naf";           // signed-digit scan of n (host_naf.hpp)
+  const bool naf = mode == "5t-naf";                            // signed-digit scan of n (host_naf.hpp)
   using O = HostOps;
   std::string sp, sn, sl;
   int count;
@@ -90,7 +91,7 @@ int main(int argc, char** argv) {
     O::s[aX] = Px; O::s[aY] = Py;
     O::s[aZ] = BigUInt(1); O::s[aZ2] = BigUInt(1);
     O::s[aF0] = BigUInt(1); O::s[aF1] = BigUInt();
-    if (five) O::s[aT5] = BigUInt(0xdead);              // must never be read or written
+    O::s[aT5] = BigUInt(0xdead);                        // must never be read or written
     std::vector<int8_t> dg = naf_digits(n);
     if (naf) {
       // self-check of the digit table: sum d_i 2^i == n, no two adjacent non-zero digits
@@ -107,20 +108,11 @@ int main(int argc, char** argv) {
     for (int m = top; m >= 0; m--) {
       const bool chord = m > 0 && (naf ? dg[m] != 0 : n.bit((size_t)m));
       const bool minus = naf && dg[m] < 0;
-      if (five) {
-        a_double_step_5t<O>();
-        if (chord)
-          a1_chord_add_5t<O>([&](int slot, int coord) { O::s[slot] = coord ? (minus ? mPy : Py) : Px; });
-      } else {
-        a_double_step<O>();
-        if (chord) {
-          O::s[aT4] = Px;
-          O::s[aT5] = minus ? mPy : Py;
-          a1_chord_add<O>(aT4, aT5);
-        }
-      }
+      a_double_step_5t<O>();
+      if (chord)
+        a1_chord_add_5t<O>([&](int slot, int coord) { O::s[slot] = coord ? (minus ? mPy : Py) : Px; });
     }
-    if (five && !(O::s[aT5] == BigUInt(0xdead))) { fprintf(stderr, "aT5 was touched\n"); return 2; }
+    if (!(O::s[aT5] == BigUInt(0xdead))) { fprintf(stderr, "aT5 was touched\n"); return 2; }
     if (pp_mode) {
       // k_a1_pp_init for P, then k_a1_pp_apply for Q: must give the same pairing
       HostTable T;

@@ -65,7 +65,6 @@ int main() {
     from_hex(p, c_fp.p, kMaxLimbs);
     c_fp.np0 = neg_inv32(c_fp.p[0]);
     c_fp.nlimbs = (uint32_t)N;
-    from_hex(d, c_fp.ninv, 5);                      // ops "fq_*split": the last argument carries -p^-1 mod 2^160
     std::string out = "?";
     if (op.rfind("fq_", 0) == 0) {
       if (N != kNS) { out = "kNS"; }
@@ -78,7 +77,6 @@ int main() {
         else if (op == "fq_mac") { FqW s, t = fq_mulw_call(A, B), u = fq_mulw_call(C, D); fqw_add(s, t, u); R = fq_redc2_call(s); }
         else if (op == "fq_mul_os") { FqW t; fqw_mul(t, A, B); fqw_redc2(R, t); }
         else if (op == "fq_mac_os") { FqW s, t, u; fqw_mul(t, A, B); fqw_mul(u, C, D); fqw_add(s, t, u); fqw_redc2(R, s); }
-        else if (op == "fq_mul_split") { FqW t; fqw_mul(t, A, B); fqw_redc_split(R, t); }
         else if (op == "fq_mul_rows") { fq_mul_os(R, A, B); }                                   // fqa_mul + fqa_merge + fqw_redc_os<false>
         else if (op == "fq_mul_rows2") { FqAcc g; FqW t; fqa_mul(g, A, B); fqa_merge<false>(t, g); fqw_redc_os<true>(R, t); }
         else if (op == "fq_acc3" || op == "fq_acc4") {

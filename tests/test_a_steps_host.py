@@ -36,7 +36,7 @@ def _run(exe, mode, pr, pairs):
     return res
 
 
-@pytest.mark.parametrize("mode", [[], ["pp"], ["5t"], ["naf"], ["5t-naf"]])
+@pytest.mark.parametrize("mode", [["pp"], ["5t"], ["5t-naf"]])
 def test_a1_slot_programs_reproduce_reference_pairings(harness, mode):
     with open(os.path.join(ROOT, "tests", "golden", "a1_small.json")) as f:
         g = json.load(f)

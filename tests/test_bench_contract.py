@@ -45,7 +45,7 @@ def test_synthetic_a1_inputs_lie_in_the_order_n_subgroup():
         for i in range(3):
             pt = pr.G1.from_bytes(bytes(buf[i * 260:(i + 1) * 260]))
             assert pt is not None and pr.E.is_valid(pt) and pr.E.mul(pr.r, pt) is None
-    assert w["exec_unit_ops_main"] == 56225715      # signed-digit scan of n (PBC_A1_NAF, default since round 2)
+    assert w["exec_unit_ops_main"] == 56225715      # signed-digit scan of n (k_a1_miller, since round 2)
 
 
 def test_parity_sample_is_seeded_distinct_and_reaches_the_last_chunk():

@@ -75,21 +75,6 @@ def test_gpu_parity_tests_pass_on_the_simulator(sim):
     assert passed >= 310, tail
 
 
-def test_kernel_variants_give_the_same_bytes(tmp_path):
-    """the compile-time variants the round-1 build measured with -- PBC_A1_SLOTS13 = 0 (six-temporary
-    programs, 96 threads per block), PBC_A1_NAF = 0 and PBC_CC_NAF = 0 (plain scans of the group order
-    in the type A1 and type F/D/G Miller loops; the default build now scans signed digits) -- and the round-2 switches of
-    the five-limb field (PBC_FQ_ACC = 0: merged products and the column-wise reduction; PBC_FS_CYC_ONE = 0: the two fused
-    cyclotomic-squaring routines; PBC_FQ_CALL_OS = 0: the column-wise out-of-line multiplier; PBC_MULW_MAD = 0; PBC_FS_ONE_QMUL = 1)
-    -- the whole battery again: both settings of every switch stay pinned"""
-    if not shutil.which("g++"):
-        pytest.skip("no g++")
-    so = _build(tmp_path, "-DPBC_A1_SLOTS13=0", "-DPBC_A1_NAF=0", "-DPBC_CC_NAF=0",
-                "-DPBC_FQ_ACC=0", "-DPBC_FS_CYC_ONE=0", "-DPBC_FQ_CALL_OS=0", "-DPBC_MULW_MAD=0", "-DPBC_FS_ONE_QMUL=1")
-    res = _battery(so)
-    assert len(res) >= 38 and all(res.values()), {k: v for k, v in res.items() if not v}
-
-
 def test_multiplier_work_counted_by_the_simulator_matches_bench(sim):
     """bench.py's roofline numerator (32x32 products the Miller kernel executes per pairing) against
     the count the PTX interpreter takes while running that kernel"""

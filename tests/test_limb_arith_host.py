@@ -137,27 +137,8 @@ def test_operand_scanning_wide_product_is_exact(harness):
     assert not bad, bad[:5]
 
 
-def test_two_product_montgomery_reduction(harness):
-    """fqw_redc_split (fq_small.cuh): m = t_lo (-q^-1) mod 2^160 on the truncated even / odd accumulators, u = m q,
-    r = t_hi + u_hi + (t_lo != 0): against Python integers, including products of unreduced operands (t up to 2 q R)
-    and t_lo = 0"""
-    rnd = random.Random(31)
-    N, R = 5, 1 << 160
-    reqs, want = [], []
-    for p in _moduli(5, 0, rnd):
-        Rinv, ninv = pow(R, -1, p), (-pow(p, -1, R)) % R
-        pairs = _operands(p, 5, rnd, 60) + [(2 * p - 1, p - 1), (R - 1, 1), (1 << 159, 2), (0, 5), (R >> 1, 2)]
-        for a, b in pairs:
-            if a * b < 2 * p * R:
-                reqs.append((N, 0, "fq_mul_split", p, a, b, 0, ninv))
-                want.append(a * b * Rinv % p)
-    got = _run(harness, reqs)
-    bad = [(hex(r[3]), hex(r[4]), hex(r[5])) for r, g, w in zip(reqs, got, want) if g != w]
-    assert len(got) == len(want) and not bad, bad[:5]
-
-
 def test_accumulating_products_and_row_wise_reduction(harness):
-    """FqAcc / fqw_redc_os (fq_small.cuh, PBC_FQ_ACC): sums of up to four 5 x 5 products kept unmerged on the even / odd
+    """FqAcc / fqw_redc_os (fq_small.cuh): sums of up to four 5 x 5 products kept unmerged on the even / odd
     accumulators with carry counts, against Python integers on the operands that drive every carry path; the row-wise
     Montgomery reduction for t < q R (one conditional subtraction) and t < 2 q R (two), including t_lo = 0, t = 0 and the
     largest inputs"""

@@ -3,7 +3,6 @@
 #   build/libpbc_b200_sim.so  -- engine.cu + every kernel compiled for the host, same C ABI
 # Use it wherever the real library would be loaded:
 #   PBC_B200_LIB=$PWD/build/libpbc_b200_sim.so python -m pytest tests/test_gpu_type_a1.py -m gpu -k "not across_blocks"
-# Extra -D flags select kernel variants, e.g.  tools/build_cpu_sim.sh -DPBC_A1_NAF=1
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p build

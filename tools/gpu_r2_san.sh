@@ -1,6 +1,5 @@
 #!/bin/bash
 mkdir -p gpurun_out
-VARIANTS="r2_default r2_q3" WL="f 524288" TAG=q3 bash tools/gpu_r2_variants.sh
 timeout 900 python -m pytest tests/test_gpu_type_a.py tests/test_gpu_type_fd.py tests/test_gpu_shim.py -m gpu -q -x 2>&1 | tail -2
 bash tools/gpu_sanitize.sh
 timeout 300 python bench.py --steps 5 --warmup 3 --workload prod16 --configs none 2>/dev/null | python -c "

@@ -137,14 +137,32 @@ __device__ __forceinline__ void g_double() {
   O::sub(gT2, gT2, gX);
   O::mulsub(gY, gT0, gT2, gT1);    // Y' = M (S - X') - 8 Y^4
 }
-// V = V + P, P affine in (gPX, gPY); V != +-P, V != O (guaranteed for scalars below r): 8 M + 3 S
-template <class O>
-__device__ __forceinline__ void g_add_affine() {
+// V = V + P, P affine in (gPX, gPY), for any V: 8 M + 3 S.  V = O (Z = 0), V = P and V = -P (H = 0)
+// happen when the order of P is not r (a point of small order, or of order p1 in type a1's composite
+// group); they take a branch of their own: V = O gives P, V = P the doubling `dbl` (the curve's
+// g_double), V = -P gives O.
+template <class O, class Dbl>
+__device__ __forceinline__ void g_add_affine(Dbl dbl) {
   O::mul(gT0, gZ2, gZ);            // Z^3
   O::mul(gT1, gPX, gZ2);
   O::sub(gT1, gT1, gX);            // H = xP Z^2 - X
   O::mul(gT0, gPY, gT0);
   O::sub(gT0, gT0, gY);            // R = yP Z^3 - Y
+  if (O::is_zero(gT1) || O::is_zero(gZ)) {
+    if (O::is_zero(gZ)) {
+      O::copy(gX, gPX);
+      O::copy(gY, gPY);
+      O::set_const(gZ, c_fp.one);
+      O::set_const(gZ2, c_fp.one);
+    } else if (O::is_zero(gT0)) {
+      dbl();
+    } else {
+      uint32_t zero[O::kVecs * O::kVecWords] = {0};
+      O::st(gZ, zero);
+      O::st(gZ2, zero);
+    }
+    return;
+  }
   O::mul(gZ, gZ, gT1);             // Z' = Z H
   O::sqr(gZ2, gZ);
   O::sqr(gT2, gT1);                // H^2
@@ -179,7 +197,7 @@ k_a_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint4* 
   O::set_const(gZ2, c_fp.one);
   for (int j = top - 1; j >= 0; j--) {
     g_double<O>();
-    if ((k[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>();
+    if ((k[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>([] { g_double<O>(); });
   }
   if (!live) return;
   uint32_t zero[kNA] = {0};
@@ -261,7 +279,7 @@ k_a_g1_from_hash(const uint8_t* __restrict__ data, int len, uint4* __restrict__ 
   O::set_const(gZ2, c_fp.one);
   for (int j = (int)c_hash.cofbits - 2; j >= 0; j--) {
     g_double<O>();
-    if ((c_hash.cofac[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>();
+    if ((c_hash.cofac[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>([] { g_double<O>(); });
   }
   if (!live) return;
   O::st_global(xyz, 0, n, idx, gX);

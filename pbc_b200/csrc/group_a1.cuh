@@ -63,7 +63,7 @@ k_a1_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, void* 
   O::set_const(gZ2, c_fp.one);
   for (int j = top - 1; j >= 0; j--) {
     g_double<O>();
-    if ((k[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>();
+    if ((k[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>([] { g_double<O>(); });
   }
   uint32_t zero[kNA1] = {0};
   if (!okP || top < 0) O::st(gZ, zero);
@@ -226,7 +226,7 @@ k_a1_g1_from_hash(const uint8_t* __restrict__ data, int len, void* __restrict__ 
   O::set_const(gZ2, c_fp.one);
   for (int j = (int)c_a1.lbits - 2; j >= 0; j--) {
     g_double<O>();
-    if ((c_a1.l[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>();
+    if ((c_a1.l[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>([] { g_double<O>(); });
   }
   O::st_global(xyz, 0, n, idx, gX);
   O::st_global(xyz, 1, n, idx, gY);

@@ -34,8 +34,7 @@ k_cc_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   X = xP;
   Y = yP;
   fq_one(Z);
-  for (int j = top - 1; j >= 0; j--) {
-    // V = 2V
+  auto dbl = [&]() {                   // V = 2V
     fq_sqr(Z2, Z);
     fq_sqr(t, X);
     fq_dbl(M, t);
@@ -62,14 +61,23 @@ k_cc_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
     fq_sub(t, t, X);
     fq_mul(Y, M, t);
     fq_sub(Y, Y, Y2);
+  };
+  for (int j = top - 1; j >= 0; j--) {
+    dbl();
     if ((k[j >> 5] >> (j & 31)) & 1u) {
-      // V = V + P (mixed)
+      // V = V + P (mixed; V = O, V = P and V = -P as in g_add_affine, group_a.cuh)
       fq_sqr(Z2, Z);
       fq_mul(t, Z2, Z);
       fq_mul(H, xP, Z2);
       fq_sub(H, H, X);
       fq_mul(R, yP, t);
       fq_sub(R, R, Y);
+      if (fq_is_zero(H) || fq_is_zero(Z)) {
+        if (fq_is_zero(Z)) { X = xP; Y = yP; fq_one(Z); }
+        else if (fq_is_zero(R)) dbl();
+        else fq_zero(Z);
+        continue;
+      }
       fq_mul(Z, H, Z);
       fq_sqr(t, H);
       fq_mul(u, t, H);
@@ -433,8 +441,7 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   X = xP;
   Y = yP;
   KF::one(Z);
-  for (int j = top - 1; j >= 0; j--) {
-    // V = 2V:  M = 3 X^2 + a' Z^4
+  auto dbl = [&]() {                   // V = 2V:  M = 3 X^2 + a' Z^4
     KF::sqr(&Z2, &Z);
     KF::sqr(&t, &X);
     KF::add(M, t, t);
@@ -460,14 +467,23 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
     KF::sub(t, t, X);
     KF::mul(&Y, &M, &t);
     KF::sub(Y, Y, Y2);
+  };
+  for (int j = top - 1; j >= 0; j--) {
+    dbl();
     if ((k[j >> 5] >> (j & 31)) & 1u) {
-      // V = V + P (mixed)
+      // V = V + P (mixed; V = O, V = P and V = -P as in g_add_affine, group_a.cuh)
       KF::sqr(&Z2, &Z);
       KF::mul(&t, &Z2, &Z);
       KF::mul(&H, &xP, &Z2);
       KF::sub(H, H, X);
       KF::mul(&R, &yP, &t);
       KF::sub(R, R, Y);
+      if (KF::is_zero(H) || KF::is_zero(Z)) {
+        if (KF::is_zero(Z)) { X = xP; Y = yP; KF::one(Z); }
+        else if (KF::is_zero(R)) dbl();
+        else Z = El();
+        continue;
+      }
       KF::mul(&Z, &H, &Z);
       KF::sqr(&t, &H);
       KF::mul(&u, &t, &H);

@@ -54,7 +54,7 @@ k_e_g1_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, void* _
   O::set_const(gZ2, c_fp.one);
   for (int j = top - 1; j >= 0; j--) {
     e_g_double<O>();
-    if ((k[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>();
+    if ((k[j >> 5] >> (j & 31)) & 1u) g_add_affine<O>([] { e_g_double<O>(); });
   }
   uint32_t zero[kNA1] = {0};
   if (!okP || top < 0) O::st(gZ, zero);

@@ -236,3 +236,17 @@ print(json.dumps(ok))
 def test_entry_points_on_the_simulator(sim, name):
     ok = _run(sim, _ENTRY_CHECK.replace("sys.argv[1]", repr(os.path.join(ROOT, "tests", "golden", "d_wide_%s.json" % name))))
     assert all(ok.values()), ok
+
+
+def test_small_order_powers_on_the_simulator(sim):
+    """the wide type D cases of tests/test_gpu_small_order_powers.py (G1 and G2 powers of points of
+    small order, against the reference fixtures and the oracle), unchanged, on the eight-limb simulator"""
+    env = dict(os.environ)
+    env["PBC_B200_LIB"] = sim
+    env["PYTHONPATH"] = ROOT + os.pathsep + env.get("PYTHONPATH", "")
+    cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider", "-k", "d_wide",
+           os.path.join(ROOT, "tests", "test_gpu_small_order_powers.py")]
+    out = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=1800, cwd=ROOT)
+    assert out.returncode == 0, out.stdout[-3000:]
+    tail = out.stdout.strip().splitlines()[-1]
+    assert int(tail.split(" passed")[0].split()[-1]) >= 8, tail

@@ -57,12 +57,13 @@ def test_every_entry_point_reproduces_the_reference_fixtures(sim):
 def test_gpu_parity_tests_pass_on_the_simulator(sim):
     """the `-m gpu` tests, unchanged, with the simulator in place of libpbc_b200.so; left out: the
     cases sized for a GPU (2^14 .. 2^18 outputs), the device-pointer entry points (they take
-    torch.cuda tensors) and the C programs of the shim (they link the real library)"""
+    torch.cuda tensors), the C programs of the shim (they link the real library) and the wide type D
+    cases (tests/test_d_wide_cpu.py runs them on the eight-limb simulator)"""
     files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_towers.py", "test_gpu_type_a.py", "test_gpu_type_a1.py",
                                                        "test_gpu_type_fd.py", "test_gpu_edge_cases.py", "test_gpu_group_ops.py",
-                                                       "test_gpu_zz_a1_group_ops.py")]
+                                                       "test_gpu_zz_a1_group_ops.py", "test_gpu_small_order_powers.py")]
     cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
-           "-k", "not large_batch and not device_pointer and not tiles and not across_blocks"] + files
+           "-k", "not large_batch and not device_pointer and not tiles and not across_blocks and not d_wide"] + files
     try:
         import xdist  # noqa: F401
         cmd += ["-n", str(max(1, min(8, len(os.sched_getaffinity(0)))))]

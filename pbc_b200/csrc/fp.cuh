@@ -269,8 +269,9 @@ __device__ __forceinline__ void redc_round(uint32_t* z, uint32_t* w, uint32_t& t
 
 // r = t / R mod p, fully reduced, for 0 <= t < 2 p R (t[0..2N], t[2N] the top word).
 // (t_lo + M p) / R <= p is formed on the even / odd accumulators (N^2 IMAD.WIDE + N IMAD), t_hi < 2p is
-// added, and the sum (< 3p) takes up to two conditional subtractions of p.
-template <int N>
+// added, and the sum (< 3p) takes up to two conditional subtractions of p.  PASSES = 1 is for t < p R (a
+// single product or square of reduced operands): t_hi < p, the sum is below 2p and one subtraction is enough.
+template <int N, int PASSES = 2>
 __device__ __forceinline__ void redc_wide(uint32_t* r, const uint32_t* t) {
   static_assert(N % 2 == 0, "even limb count");
   uint32_t x[N], y[N], top;
@@ -294,7 +295,7 @@ __device__ __forceinline__ void redc_wide(uint32_t* r, const uint32_t* t) {
   for (int k = 1; k < N; k++) PBC_ASM("addc.cc.u32 %0, %0, %1;" : "+r"(s[k]) : "r"(t[N + k]));
   PBC_ASM("addc.u32 %0, %0, %1;" : "+r"(top) : "r"(t[2 * N]));
 #pragma unroll
-  for (int pass = 0; pass < 2; pass++) {
+  for (int pass = 0; pass < PASSES; pass++) {
     uint32_t d[N], dtop;
     PBC_ASM("sub.cc.u32 %0, %1, %2;" : "=r"(d[0]) : "r"(s[0]), "r"(c_fp.p[0]));
 #pragma unroll
@@ -308,6 +309,106 @@ __device__ __forceinline__ void redc_wide(uint32_t* r, const uint32_t* t) {
   }
 #pragma unroll
   for (int k = 0; k < N; k++) r[k] = s[k];
+}
+
+// ---------------------------------------------------------------------------------------------
+// Row-wise squaring on the even / odd accumulators.  The cross products a_i a_j (i < j) are summed once,
+// every one of them a single IMAD.WIDE.U32 with the carry in the flag, the sum is doubled by one carry chain
+// and the diagonal a_i^2 is added as one run of N adjacent pairs: N(N-1)/2 + N products and about 3 N
+// additions per limb pair, against N(N+1)/2 products each followed by an IADD3.X plus the per-column
+// bookkeeping of the product-scanning squarer.
+//
+// Accumulators are indexed by absolute column: the pair (e[c], e[c+1]), c even, and (o[c], o[c+1]), c odd,
+// receive the products whose low word lands on column c.  Row i holds a_i a_j for j = i+1 .. N-1: its odd
+// chain starts at column 2i+1, its even chain at 2i+2, and its top product a_i a_{N-1} opens a new pair at
+// column T = i+N-1.  The sum of rows 0..i is below 2^(32(i+N+1)), so nothing is carried beyond column T+1:
+// the chain that does not own the new pair hands its carry to that pair's high word.  Columns 2i-1 and 2i
+// are complete when row i starts; e and o are merged there and the merge carry enters the odd chain, so the
+// live window shrinks as the finished words of p grow.
+// ---------------------------------------------------------------------------------------------
+template <int N, int I>
+__device__ __forceinline__ void sqr_cross_row(uint32_t* p, uint32_t* e, uint32_t* o, const uint32_t* a) {
+  constexpr int T = I + N - 1;
+  constexpr bool kTopOdd = (T & 1) != 0;
+  if constexpr (I == 0) {
+    // nothing to add to yet: plain products
+#pragma unroll
+    for (int c = 1; c <= T; c += 2)
+      PBC_ASM("mul.lo.u32 %0, %2, %3; mul.hi.u32 %1, %2, %3;" : "=r"(o[c]), "=r"(o[c + 1]) : "r"(a[0]), "r"(a[c]));
+#pragma unroll
+    for (int c = 2; c <= T; c += 2)
+      PBC_ASM("mul.lo.u32 %0, %2, %3; mul.hi.u32 %1, %2, %3;" : "=r"(e[c]), "=r"(e[c + 1]) : "r"(a[0]), "r"(a[c]));
+  } else {
+    if constexpr (I == 1) {
+      p[0] = 0;                 // no cross product lands on columns 0 and 1 of e
+      p[1] = o[1];
+      PBC_ASM("add.cc.u32 %0, %1, %2;" : "=r"(p[2]) : "r"(e[2]), "r"(o[2]));
+    } else {
+      PBC_ASM("add.cc.u32 %0, %1, %2;" : "=r"(p[2 * I - 1]) : "r"(e[2 * I - 1]), "r"(o[2 * I - 1]));
+      PBC_ASM("addc.cc.u32 %0, %1, %2;" : "=r"(p[2 * I]) : "r"(e[2 * I]), "r"(o[2 * I]));
+    }
+    // odd columns: the merge carry enters at column 2I+1
+#pragma unroll
+    for (int c = 2 * I + 1; c <= T; c += 2) {
+      if (c == T)
+        PBC_ASM("madc.lo.cc.u32 %0, %2, %3, 0; madc.hi.cc.u32 %1, %2, %3, 0;"
+                : "=r"(o[c]), "=r"(o[c + 1]) : "r"(a[I]), "r"(a[c - I]));
+      else
+        PBC_ASM("madc.lo.cc.u32 %0, %2, %3, %0; madc.hi.cc.u32 %1, %2, %3, %1;"
+                : "+r"(o[c]), "+r"(o[c + 1]) : "r"(a[I]), "r"(a[c - I]));
+    }
+    uint32_t t = 0;
+    if constexpr (!kTopOdd) t = carry_out();     // out of column T: the high word of the even chain's new pair
+    // even columns
+#pragma unroll
+    for (int c = 2 * I + 2; c <= T; c += 2) {
+      if (c == T && c == 2 * I + 2)
+        PBC_ASM("mul.lo.u32 %0, %2, %3; mad.hi.u32 %1, %2, %3, %4;"
+                : "=r"(e[c]), "=r"(e[c + 1]) : "r"(a[I]), "r"(a[c - I]), "r"(t));
+      else if (c == T)
+        PBC_ASM("madc.lo.cc.u32 %0, %2, %3, 0; madc.hi.u32 %1, %2, %3, %4;"
+                : "=r"(e[c]), "=r"(e[c + 1]) : "r"(a[I]), "r"(a[c - I]), "r"(t));
+      else if (c == 2 * I + 2)
+        PBC_ASM("mad.lo.cc.u32 %0, %2, %3, %0; madc.hi.cc.u32 %1, %2, %3, %1;"
+                : "+r"(e[c]), "+r"(e[c + 1]) : "r"(a[I]), "r"(a[c - I]));
+      else
+        PBC_ASM("madc.lo.cc.u32 %0, %2, %3, %0; madc.hi.cc.u32 %1, %2, %3, %1;"
+                : "+r"(e[c]), "+r"(e[c + 1]) : "r"(a[I]), "r"(a[c - I]));
+    }
+    if constexpr (kTopOdd && 2 * I + 2 < T) PBC_ASM("addc.u32 %0, %0, 0;" : "+r"(o[T + 1]));
+  }
+  if constexpr (I + 2 < N) sqr_cross_row<N, I + 1>(p, e, o, a);
+}
+
+// p[0..2N) = a^2, exact.
+template <int N>
+__device__ __forceinline__ void sqr_wide(uint32_t* p, const uint32_t* a) {
+  static_assert(N % 2 == 0 && N >= 4, "even limb count");
+  uint32_t e[2 * N], o[2 * N];
+  sqr_cross_row<N, 0>(p, e, o, a);
+  // the last row (I = N-2) left columns 2N-3 and 2N-2; no pair of e reaches column 2N-2
+  PBC_ASM("add.cc.u32 %0, %1, %2;" : "=r"(p[2 * N - 3]) : "r"(e[2 * N - 3]), "r"(o[2 * N - 3]));
+  PBC_ASM("addc.cc.u32 %0, %1, 0;" : "=r"(p[2 * N - 2]) : "r"(o[2 * N - 2]));
+  PBC_ASM("addc.u32 %0, 0, 0;" : "=r"(p[2 * N - 1]));
+  // p = 2 p + sum a_i^2 2^(64 i)
+  PBC_ASM("add.cc.u32 %0, %0, %0;" : "+r"(p[1]));
+#pragma unroll
+  for (int k = 2; k < 2 * N - 1; k++) PBC_ASM("addc.cc.u32 %0, %0, %0;" : "+r"(p[k]));
+  PBC_ASM("addc.u32 %0, %0, %0;" : "+r"(p[2 * N - 1]));
+  PBC_ASM("mad.lo.cc.u32 %0, %2, %2, %0; madc.hi.cc.u32 %1, %2, %2, %1;" : "+r"(p[0]), "+r"(p[1]) : "r"(a[0]));
+#pragma unroll
+  for (int i = 1; i < N; i++)
+    PBC_ASM("madc.lo.cc.u32 %0, %2, %2, %0; madc.hi.cc.u32 %1, %2, %2, %1;"
+            : "+r"(p[2 * i]), "+r"(p[2 * i + 1]) : "r"(a[i]));
+}
+
+// r = a^2/R mod p, input and output fully reduced.  r may alias a.  a^2 < p R: one conditional subtraction.
+template <int N>
+__device__ __forceinline__ void mont_sqr_os(uint32_t* r, const uint32_t* a) {
+  uint32_t t[2 * N + 1];
+  sqr_wide<N>(t, a);
+  t[2 * N] = 0;
+  redc_wide<N, 1>(r, t);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -420,17 +521,17 @@ __device__ __forceinline__ void mont_sqr_ps(uint32_t* r, const uint32_t* a) {
   for (int k = 0; k < N; k++) r[k] = use_d ? d[k] : t[k];
 }
 
-// The multiplier the kernels use.  Where IMAD.WIDE.U32 issues at the same rate with or without
-// carries, the two multipliers execute the same number of multiplier-pipe slots; operand scanning has
-// about a quarter fewer ALU instructions and suits a*b, product scanning suits a^2 (408 instead of 528
-// IMAD.WIDE): operand scanning for products, product scanning for squares.
+// The multiplier the kernels use.  Operand scanning for products.  For squares the 16-limb full-width field
+// (type A) takes the row-wise squarer, whose additions ride on the carry flag of the products; the other
+// widths keep product scanning.  Both squarers issue N(N+1)/2 + N^2 IMAD.WIDE (408 for N = 16, against 528).
 template <int N, bool FULL>
 __device__ __forceinline__ void fp_mul(uint32_t* r, const uint32_t* a, const uint32_t* b) {
   mont_mul<N, FULL>(r, a, b);
 }
 template <int N, bool FULL>
 __device__ __forceinline__ void fp_sqr(uint32_t* r, const uint32_t* a) {
-  mont_sqr_ps<N, FULL>(r, a);
+  if constexpr (N == 16 && FULL) mont_sqr_os<N>(r, a);
+  else mont_sqr_ps<N, FULL>(r, a);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -44,11 +44,11 @@ __device__ __forceinline__ bool a_load_point(int sx, int sy, int st0, int st1, c
   limbs_from_be<kNA, kWA>(x, p + kWA);
   mont_mul<kNA, true>(x, x, c_fp.r2);
   O::st(sy, x);
-  O::sqr(st0, sx);
+  O::sqrp(st0, sx);
   O::set_const(st1, c_fp.one);
   O::add(st0, st0, st1);      // x^2 + 1
   O::mul(st0, st0, sx);       // x^3 + x
-  O::sqr(st1, sy);
+  O::sqrp(st1, sy);
   return O::eq(st0, st1) && !O::is_zero(sy);
 }
 
@@ -80,9 +80,9 @@ enum A9Slot { nX, nY, nZ, nF0, nF1, nT0, nT1, nT2, nT3, kA9Slots };
 // per SM), k_a_miller9_shared keeps more live across its calls and does not, so it runs LAZY = false.
 template <class O, bool LAZY>
 __device__ __forceinline__ void a_step_9_line(const uint4* qx, const uint4* qy, size_t n) {
-  O::sqr(nT1, nX);                                   // A
-  O::sqr(nT2, nY);                                   // B
-  O::sqr(nT3, nZ);                                   // C
+  O::sqrp(nT1, nX);                                   // A
+  O::sqrp(nT2, nY);                                   // B
+  O::sqrp(nT3, nZ);                                   // C
   O::sub(nF0, nT1, nT3);                             // T = A - C
   O::add(nT3, nT1, nT3);                             // A' = A + C
   O::dbl(nT1, nT3);
@@ -95,14 +95,9 @@ __device__ __forceinline__ void a_step_9_line(const uint4* qx, const uint4* qy, 
     O::mulp(nX, nX, nF0);                            // X T
     O::add(nT1, nT1, nX);                            // Re l                   (X slot is free)
   }
-  O::sqr(nX, nF0);                                   // X' = T^2
-  O::sqr(nT3, nT3);
-  O::dbl(nT3, nT3);
-  O::sub(nT3, nT3, nX);                              // E = 2 A'^2 - X'
-  O::add(nF0, nF0, nY);
-  O::sqr(nF0, nF0);
-  O::sub(nF0, nF0, nT2);
-  O::sub(nF0, nF0, nX);                              // F = (T + Y)^2 - B - X'
+  O::sqrp(nX, nF0);                                  // X' = T^2
+  O::sqrx(nT3, nT3, O::SX_SUB_1, 0, 1, nX, 0);       // E = 2 A'^2 - X'
+  O::sqrx(nF0, nF0, O::SX_ADD_A | O::SX_SUB_1 | O::SX_SUB_2, nY, 0, nT2, nX);   // F = (T + Y)^2 - B - X'
   O::mulp(nT3, nT3, nF0);                            // Y' (kept in T3 until Y has had its last use)
   O::mulp(nF0, nY, nZ);
   O::dbl(nF0, nF0);
@@ -168,9 +163,9 @@ __device__ __forceinline__ void a_chord_line(int x, int y, int z, int t0, int t1
   O::mulp(t1, t1, t0);                          // X1 Z1
   O::mulp(t1, t1, y);                           // Y X1 Z1
   O::sub(t3, t3, t1);                           // c
-  O::sqr(t0, t0);                               // Z1^2
+  O::sqrp(t0, t0);                               // Z1^2
   O::mulp(t0, t0, y);                           // Y Z1^2
-  O::sqr(t1, z);                                // Z^2
+  O::sqrp(t1, z);                                // Z^2
   O::mulp(t1, t1, x);                           // Y1 Z^2
   O::sub(t0, t0, t1);                           // a
   O::mulg(t0, t0, qx, n);
@@ -233,8 +228,8 @@ k_a_miller9(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q, uint4*
   a_chord_9<O>(save, qx, qy, n, idx);
 
   // D = (f0^2 + f1^2) f0 f1;  invalid inputs publish D = 0 (-> identity)
-  O::sqr(nT0, nF0);
-  O::sqr(nT1, nF1);
+  O::sqrp(nT0, nF0);
+  O::sqrp(nT1, nF1);
   O::add(nT0, nT0, nT1);
   O::mulp(nT1, nF0, nF1);
   O::mulp(nT0, nT0, nT1);
@@ -326,8 +321,8 @@ k_a_miller9_shared(const uint8_t* __restrict__ P, const uint8_t* __restrict__ Q,
     O::ld_global(nZ, vj, 2, np, pr);
     a_chord_9<O>(save, qm + pr, qm + 4 * np + pr, np, pr);
   }
-  O::sqr(nT0, nF0);
-  O::sqr(nT1, nF1);
+  O::sqrp(nT0, nF0);
+  O::sqrp(nT1, nF1);
   O::add(nT0, nT0, nT1);
   O::mulp(nT1, nF0, nF1);
   O::mulp(nT0, nT0, nT1);
@@ -367,8 +362,8 @@ k_a_prod(const uint4* __restrict__ f_in, const uint4* __restrict__ d_in, uint4* 
     valid = valid && !O::is_zero(pT0);
     a_fmul<O>(pF0, pF1, pL0, pL1, pT0, pT1, pT2);
   }
-  O::sqr(pT0, pF0);
-  O::sqr(pT1, pF1);
+  O::sqrp(pT0, pF0);
+  O::sqrp(pT1, pF1);
   O::add(pT0, pT0, pT1);
   O::mul(pT1, pF0, pF1);
   O::mul(pT0, pT0, pT1);
@@ -412,12 +407,12 @@ k_a_pp_init(const uint8_t* __restrict__ P, uint32_t* __restrict__ tab) {
     }
     // tangent (compute_abc_tangent_proj, ecc/a_param.c:86-112), sign-flipped as a whole:
     //   a = M Z^2, b = 2 Y Z^3, c = X M - 2 Y^2     with M = 3 X^2 + Z^4;  line = c + a Qx... see apply
-    O::sqr(aT0, aX);
-    O::sqr(aT1, aZ2);
+    O::sqrp(aT0, aX);
+    O::sqrp(aT1, aZ2);
     O::dbl(aT2, aT0);
     O::add(aT0, aT0, aT2);
     O::add(aT0, aT0, aT1);          // M
-    O::sqr(aT1, aY);                // Y^2
+    O::sqrp(aT1, aY);                // Y^2
     O::mul(aT3, aT0, aZ2);          // a = M Z^2
     emit(3 * i + 0, aT3);
     O::mul(aT5, aX, aT0);
@@ -430,11 +425,11 @@ k_a_pp_init(const uint8_t* __restrict__ P, uint32_t* __restrict__ tab) {
     O::dbl(aZ, aZ);                 // Z' = 2 Y Z
     O::mul(aT3, aZ, aZ2);           // b = Z' Z^2
     emit(3 * i + 1, aT3);
-    O::sqr(aZ2, aZ);
-    O::sqr(aT5, aT0);
+    O::sqrp(aZ2, aZ);
+    O::sqrp(aT5, aT0);
     O::sub(aX, aT5, aT2);
     O::sub(aX, aX, aT2);            // X' = M^2 - 2 S
-    O::sqr(aT1, aT1);
+    O::sqrp(aT1, aT1);
     O::dbl(aT1, aT1, 3);            // 8 Y^4
     O::sub(aT2, aT2, aX);
     O::mulsub(aY, aT0, aT2, aT1);   // Y' = M (S - X') - 8 Y^4
@@ -442,7 +437,7 @@ k_a_pp_init(const uint8_t* __restrict__ P, uint32_t* __restrict__ tab) {
   // chord through V = (X, Y, Z) and V1 = (X1, Y1, Z1), scaled by Z^3 Z1^3 (compute_abc_line :114-130)
   //   a = Y Z1^3 - Y1 Z^3,  b = X1 Z1 Z^3 - X Z Z1^3,  c = X Z Y1 - Y X1 Z1
   O::mul(aT1, aZ2, aZ);             // Z^3
-  O::sqr(aT2, aF0);
+  O::sqrp(aT2, aF0);
   O::mul(aT2, aT2, aF0);            // Z1^3
   O::mul(aT3, aX, aZ);              // X Z
   O::mul(aT4, aQX, aF0);            // X1 Z1
@@ -504,8 +499,8 @@ k_a_pp_apply(const uint32_t* __restrict__ tab, const uint8_t* __restrict__ Q, ui
     a_fmul<O>(qF0, qF1, qT0, qT1, qT2, qT3, qT4);
   }
   if (!live) return;
-  O::sqr(qT0, qF0);
-  O::sqr(qT1, qF1);
+  O::sqrp(qT0, qF0);
+  O::sqrp(qT1, qF1);
   O::add(qT0, qT0, qT1);
   O::mul(qT1, qF0, qF1);
   O::mul(qT0, qT0, qT1);

@@ -118,6 +118,31 @@ struct Ops {
   }
   static __device__ __forceinline__ void mulp(int d, int a, int b) { mulx(d, a, b, 0, 0, 0, nullptr, 0); }
 
+  // ---- ONE squaring routine with its additions folded in, as mulx is for products ----
+  //   d = 2^k (a [+ a2])^2 [- s1] [- s2]
+  // Each folded addition is a separate out-of-line call less: a shared-memory round trip of its operands during
+  // which the warp feeds the multiplier nothing.  Every intermediate is fully reduced, so d is the value the
+  // separate calls give.  All branches are warp-uniform; d may alias any operand.
+  static constexpr uint32_t SX_ADD_A = 1u, SX_SUB_1 = 2u, SX_SUB_2 = 4u;
+  static __device__ __noinline__ void sqrx(int d, int a, uint32_t mode, int a2, int k, int s1, int s2) {
+    uint32_t x[N], y[N];
+    ld(x, a);
+    if (mode & SX_ADD_A) {
+      ld(y, a2);
+      fp_add<N, FULL>(x, x, y);
+    }
+    fp_sqr<N, FULL>(x, x);
+    for (int i = 0; i < k; i++) fp_add<N, FULL>(x, x, x);
+    const int subs = (mode & SX_SUB_1) ? ((mode & SX_SUB_2) ? 2 : 1) : 0;
+#pragma unroll 1
+    for (int i = 0; i < subs; i++) {
+      ld(y, i ? s2 : s1);
+      fp_sub<N>(x, x, y);
+    }
+    st(d, x);
+  }
+  static __device__ __forceinline__ void sqrp(int d, int a) { sqrx(d, a, 0, 0, 0, 0, 0); }
+
   // ---- lazy reduction (fp.cuh mul_wide / redc_wide; FULL, even N) ----
   //   d = (a0 b0 [+- a1 b1] [+ q R] [- S]) / R mod q,   S = the unreduced value in slots (s0, s1)
   // One Montgomery reduction for the whole sum: a second product costs N^2 IMAD.WIDE, not N^2 + N^2 + N.

@@ -2303,6 +2303,70 @@ k_fp_op(int op, uint8_t* __restrict__ out, const uint8_t* __restrict__ a, const 
   mont_mul<N, FULL>(x, x, one);
   limbs_to_be<N, WB>(out + idx * WB, x);
 }
+// Ops 8-14 of the type A hook: the slot routines of the Miller step (a_step_9_line, pairing_a.cuh) in its call
+// sequences and with its mode flags; coordinates per item (in a, in b, in out) from fp_op_widths, a = (a0, a1),
+// b = (b0, b1):
+//    8  lazy(LZ_TWO | LZ_GLOBAL_B), b0 read from a limb-major global array as qx is:  a0 b0 + a1 b1
+//    9  lazy(LZ_TWO | LZ_SUB | LZ_ADD_QR | LZ_KARATSUBA) then lazy(LZ_SUB_S | LZ_ADD_QR) on the stored S':
+//       out = (a0 b0 - a1 b1, a0 b1 + a1 b0, S' low half, S' high half, a0 + a1, b0 + b1); the two halves of
+//       S' are the raw 512-bit slot words (S' = A0 B0 + A1 B1, less q R if that is >= q R, A = a R mod q)
+//   10  sqrx(SX_SUB_1, k = 1):                          2 a0^2 - b0
+//   11  sqrx(SX_ADD_A | SX_SUB_1 | SX_SUB_2):           (a0 + a1)^2 - b0 - b1
+//   12  mulx(MX_ADD_A | MX_ADD_B):                      (a0 + a1)(b0 + b1)
+//   13  mulx(MX_ADD_A | MX_SUB_B):                      (a0 + a1)(b0 - b1)
+//   14  mulx(MX_GLOBAL_B):                              a0 b0, b0 from the global array
+// It runs in 64-thread blocks: an instantiation of the slot routines of its own, so that calling them from here
+// leaves the code ptxas makes for the shipped 128-thread kernels as it is (the routines are shared, and their
+// callers' constant mode arguments shape that code).  g: scratch for b0, N / 4 vectors per item, n apart.
+__host__ __device__ inline void fp_op_widths(int op, int* wa, int* wb, int* wo) {
+  *wa = (op == 8 || op == 9 || op == 11 || op == 12 || op == 13) ? 2 : 1;
+  *wb = (op == 10 || op == 14 || op < 8) ? 1 : 2;
+  *wo = op == 9 ? 6 : 1;
+}
+template <int N, int WB, int BLOCK>
+__global__ void __launch_bounds__(BLOCK)
+k_fp_slot_op(int op, uint8_t* __restrict__ out, const uint8_t* __restrict__ a, const uint8_t* __restrict__ b,
+             uint4* __restrict__ g, size_t n) {
+  using O = Ops<N, true, BLOCK>;
+  size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
+  if (idx >= n) return;
+  int wa, wb, wo;
+  fp_op_widths(op, &wa, &wb, &wo);
+  uint32_t x[N], one[N] = {1};
+  // coordinate c of a into slot 2c, of b into slot 2c + 1, Montgomery form
+  for (int c = 0; c < wa + wb; c++) {
+    const bool isa = c < wa;
+    limbs_from_be<N, WB>(x, isa ? a + (idx * wa + c) * WB : b + (idx * wb + c - wa) * WB);
+    mont_mul<N, true>(x, x, c_fp.r2);
+    O::st(isa ? 2 * c : 2 * (c - wa) + 1, x);
+  }
+  if (op == 8 || op == 14) {
+    O::ld(x, 1);
+#pragma unroll
+    for (int v = 0; v < N / 4; v++) g[v * n + idx] = make_uint4(x[4 * v], x[4 * v + 1], x[4 * v + 2], x[4 * v + 3]);
+  }
+  int res[6] = {0, 0, 0, 0, 0, 0};
+  bool raw[6] = {false, false, false, false, false, false};
+  switch (op) {    // slot aliasing as in a_step_9_line: the result overwrites an operand
+    case 8: O::lazy(0, O::LZ_TWO | O::LZ_GLOBAL_B, 0, 0, 2, 3, 0, 0, g + idx, n); break;
+    case 9:
+      O::lazy(3, O::LZ_TWO | O::LZ_SUB | O::LZ_ADD_QR | O::LZ_KARATSUBA, 0, 1, 2, 3, 4, 5, nullptr, 0);
+      O::lazy(2, O::LZ_SUB_S | O::LZ_ADD_QR, 0, 1, 0, 0, 4, 5, nullptr, 0);
+      res[0] = 3; res[1] = 2; res[2] = 4; res[3] = 5; res[4] = 0; res[5] = 1;
+      raw[2] = raw[3] = true;
+      break;
+    case 10: O::sqrx(0, 0, O::SX_SUB_1, 0, 1, 1, 0); break;
+    case 11: O::sqrx(0, 0, O::SX_ADD_A | O::SX_SUB_1 | O::SX_SUB_2, 2, 0, 1, 3); break;
+    case 12: O::mulx(0, 0, 1, O::MX_ADD_A | O::MX_ADD_B, 2, 3, nullptr, 0); break;
+    case 13: O::mulx(0, 0, 1, O::MX_ADD_A | O::MX_SUB_B, 2, 3, nullptr, 0); break;
+    default: O::mulx(0, 0, 0, O::MX_GLOBAL_B, 0, 0, g + idx, n); break;
+  }
+  for (int c = 0; c < wo; c++) {
+    O::ld(x, res[c]);
+    if (!raw[c]) mont_mul<N, true>(x, x, one);
+    limbs_to_be<N, WB>(out + (idx * wo + c) * WB, x);
+  }
+}
 // same hook for the five-limb field of types f and d
 template <int W>
 __global__ void k_fq_op(int op, uint8_t* __restrict__ out, const uint8_t* __restrict__ a,
@@ -2370,15 +2434,25 @@ extern "C" int pbc_b200_fp_op(pbc_b200_pairing_t* p, int op, unsigned char* out,
   std::lock_guard<std::mutex> dev_lock(g_dev_mu[dev & 63]);
   if (ctx_prepare(p, dev)) return 1;
   size_t wb = (size_t)p->g1_len / 2;             // bytes per F_q coordinate: 64, 20, 19 or ceil(bits(p)/8)
-  DevBuf da, db, dout;
-  CUDA_OK(da.alloc(n * wb));
-  CUDA_OK(db.alloc(n * wb));
-  CUDA_OK(dout.alloc(n * wb));
-  CUDA_OK(cudaMemcpy(da.p, a, n * wb, cudaMemcpyHostToDevice));
-  CUDA_OK(cudaMemcpy(db.p, b ? b : a, n * wb, cudaMemcpyHostToDevice));
+  int wa = 1, wbn = 1, wo = 1;                   // coordinates per item (type a ops 8-14: see fp_op_widths)
+  if (p->type == 'a') {
+    if (op < 0 || op > 14) return fail("fp_op: type a has ops 0..14");
+    fp_op_widths(op, &wa, &wbn, &wo);
+  }
+  if (wbn > 1 && !b) return fail("fp_op %d: needs b", op);
+  DevBuf da, db, dout, dg;
+  CUDA_OK(da.alloc(n * wb * wa));
+  CUDA_OK(db.alloc(n * wb * wbn));
+  CUDA_OK(dout.alloc(n * wb * wo));
+  CUDA_OK(cudaMemcpy(da.p, a, n * wb * wa, cudaMemcpyHostToDevice));
+  CUDA_OK(cudaMemcpy(db.p, b ? b : a, n * wb * wbn, cudaMemcpyHostToDevice));
   unsigned g = (unsigned)((n + 127) / 128);
   if (p->type == '1' || p->type == 'e') {
     k_a1_fp_op<kBlockA1Small><<<g, kBlockA1Small, (size_t)4 * kSlotA1 * kBlockA1Small>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
+  } else if (p->type == 'a' && op >= 8) {
+    CUDA_OK(dg.alloc(n * wb));                   // b0 of ops 8 and 14 as a limb-major global array
+    k_fp_slot_op<kNA, 64, 64><<<(unsigned)((n + 63) / 64), 64, 6 * 64 * 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(),
+                                                                          db.as<uint8_t>(), dg.as<uint4>(), n);
   } else if (p->type == 'a') {
     CUDA_OK(allow_smem(k_fp_op<kNA, true, 64, 128>, 4 * 64 * 128));
     k_fp_op<kNA, true, 64, 128><<<g, 128, 4 * 64 * 128>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
@@ -2391,7 +2465,7 @@ extern "C" int pbc_b200_fp_op(pbc_b200_pairing_t* p, int op, unsigned char* out,
   }
   LAUNCHED();
   CUDA_OK(cudaDeviceSynchronize());
-  CUDA_OK(cudaMemcpy(out, dout.p, n * wb, cudaMemcpyDeviceToHost));
+  CUDA_OK(cudaMemcpy(out, dout.p, n * wb * wo, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -2413,6 +2487,24 @@ extern "C" int pbc_b200_tower_op(pbc_b200_pairing_t* p, int op, unsigned char* o
   CUDA_OK(cudaMemcpy(da.p, a, n * wb, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(db.p, b ? b : a, n * wb, cudaMemcpyHostToDevice));
   unsigned g = (unsigned)((n + 63) / 64);
+  if (op == 6 && p->type == 'f') {
+    // the final exponentiation every type F pairing takes (k_f_finalexp_s), on the caller's elements: they
+    // go into the Miller-value layout with their flags set, then the launch of enqueue_pairings
+    if (!(p->f.slots_ok && p->f.bn))
+      return fail("tower_op 6: the slot-machine final exponentiation needs the internal basis and a BN parameter");
+    DevBuf ws;
+    CUDA_OK(ws.alloc(n * 4 * ((size_t)kF12Words + 1 + (size_t)kFStashWords)));
+    uint32_t* mv = ws.as<uint32_t>();
+    uint32_t* flag = mv + (size_t)kF12Words * n;
+    uint32_t* stash = flag + n;
+    k_f_mv_from_wire<<<g, 64>>>(mv, flag, da.as<uint8_t>(), n);
+    LAUNCHED();
+    k_f_finalexp_s<kBlockFS><<<(unsigned)((n + kBlockFS - 1) / kBlockFS), kBlockFS, kSmemFFinalS>>>(mv, flag, dout.as<uint8_t>(), stash, n);
+    LAUNCHED();
+    CUDA_OK(cudaDeviceSynchronize());
+    CUDA_OK(cudaMemcpy(out, dout.p, n * wb, cudaMemcpyDeviceToHost));
+    return 0;
+  }
   if (p->dwide) pbcb200_dw::dw_tower_op(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n, 0);
   else if (p->type == 'f') k_f_tower_op<<<g, 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);
   else if (p->type == 'g') k_g_tower_op<<<g, 64>>>(op, dout.as<uint8_t>(), da.as<uint8_t>(), db.as<uint8_t>(), n);

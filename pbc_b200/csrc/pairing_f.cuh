@@ -699,5 +699,17 @@ __global__ void k_f_tower_op(int op, uint8_t* __restrict__ out, const uint8_t* _
   f12_to_reference(r);
   f12_to_wire(out + idx * (12 * kWS), r);
 }
+// test hook of tower op 6: GT wire elements into the limb-major Miller-value layout k_f_finalexp and
+// k_f_finalexp_s read (internal basis, Montgomery form), every flag set
+__global__ void k_f_mv_from_wire(uint32_t* __restrict__ mv, uint32_t* __restrict__ flag, const uint8_t* __restrict__ a,
+                                 size_t n) {
+  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  F12 x;
+  f12_from_wire(x, a + idx * (12 * kWS));
+  f12_to_internal(x);
+  f12_st_global(mv, n, idx, x);
+  flag[idx] = 1u;
+}
 
 }  // namespace pbcb200

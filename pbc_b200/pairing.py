@@ -247,12 +247,17 @@ class Pairing:
             raise PairingError(last_error())
 
     # -- test / bench hooks -----------------------------------------------------------------------
-    def fp_op(self, op: int, a: bytes, b, n: int) -> bytes:
+    def fp_op(self, op: int, a: bytes, b, n: int, widths=(1, 1, 1)) -> bytes:
+        """widths: coordinates per item in a, b and the result (type a ops 8-14 take several, see
+        pbc_b200_fp_op); the library knows them per op, they size and check the buffers here"""
         wb = self.g1_len // 2          # bytes per F_q coordinate
-        out = C.create_string_buffer(n * wb)
+        self._need(a, n * wb * widths[0], "fp_op a")
+        if b is not None:
+            self._need(b, n * wb * widths[1], "fp_op b")
+        out = C.create_string_buffer(max(1, n * wb * widths[2]))
         if lib.pbc_b200_fp_op(self._h, op, C.addressof(out), _addr(a), _addr(b), n):
             raise PairingError(last_error())
-        return out.raw
+        return out.raw[:n * wb * widths[2]]
 
     def tower_op(self, op: int, a: bytes, b, n: int) -> bytes:
         out = C.create_string_buffer(n * self.gt_len)

@@ -250,3 +250,18 @@ def test_small_order_powers_on_the_simulator(sim):
     assert out.returncode == 0, out.stdout[-3000:]
     tail = out.stdout.strip().splitlines()[-1]
     assert int(tail.split(" passed")[0].split()[-1]) >= 8, tail
+
+
+def test_montgomery_extremes_on_the_simulator(sim):
+    """the wide type D cases of tests/test_gpu_montgomery_extremes.py (field ops, square roots and the F_q^3 /
+    F_q^6 tower on operands extreme in the Montgomery domain, both bases), unchanged, on the eight-limb
+    simulator"""
+    env = dict(os.environ)
+    env["PBC_B200_LIB"] = sim
+    env["PYTHONPATH"] = ROOT + os.pathsep + env.get("PYTHONPATH", "")
+    cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider", "-k", "d_wide",
+           os.path.join(ROOT, "tests", "test_gpu_montgomery_extremes.py")]
+    out = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=1800, cwd=ROOT)
+    assert out.returncode == 0, out.stdout[-3000:]
+    tail = out.stdout.strip().splitlines()[-1]
+    assert int(tail.split(" passed")[0].split()[-1]) >= 18, tail

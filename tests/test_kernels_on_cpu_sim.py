@@ -61,7 +61,8 @@ def test_gpu_parity_tests_pass_on_the_simulator(sim):
     cases (tests/test_d_wide_cpu.py runs them on the eight-limb simulator)"""
     files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_towers.py", "test_gpu_type_a.py", "test_gpu_type_a1.py",
                                                        "test_gpu_type_fd.py", "test_gpu_edge_cases.py", "test_gpu_group_ops.py",
-                                                       "test_gpu_zz_a1_group_ops.py", "test_gpu_small_order_powers.py")]
+                                                       "test_gpu_zz_a1_group_ops.py", "test_gpu_small_order_powers.py",
+                                                       "test_gpu_montgomery_extremes.py")]
     cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
            "-k", "not large_batch and not device_pointer and not tiles and not across_blocks and not d_wide"] + files
     try:

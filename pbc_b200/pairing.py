@@ -242,6 +242,10 @@ class Pairing:
         if lib.pbc_b200_g1_pow_zn_device(self._h, d_out, d_in, d_k, n, stream):
             raise PairingError(last_error())
 
+    def g2_pow_zn_device(self, d_out, d_in, d_k, n, stream=0):
+        if lib.pbc_b200_g2_pow_zn_device(self._h, d_out, d_in, d_k, n, stream):
+            raise PairingError(last_error())
+
     def gt_pow_zn_device(self, d_out, d_in, d_k, n, stream=0):
         if lib.pbc_b200_gt_pow_zn_device(self._h, d_out, d_in, d_k, n, stream):
             raise PairingError(last_error())

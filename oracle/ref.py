@@ -72,6 +72,12 @@ class RefPairing:
         self.g1_len, self.g2_len, self.gt_len, self.zr_len = list(sz)
         self.last_seconds = 0.0
 
+    def close(self):
+        """pairing_clear; the handle is unusable afterwards"""
+        if self.h:
+            self.L.pbcref_close(self.h)
+            self.h = None
+
     def _len(self, group):
         return {G1: self.g1_len, G2: self.g2_len, GT: self.gt_len, ZR: self.zr_len}[group]
 

@@ -255,13 +255,19 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
   if (job.mode == kProd) bytes += n_out * (W + 1) * 4;
   return bytes;
 }
+// G1's cofactor (fill_hash) is 1: every point of E(F_q) has order r
+static bool g1_cofactor_one(const pbc_b200_pairing_s* p) {
+  for (int i = 1; i < 12; i++)
+    if (p->hash.cofac[i]) return false;
+  return p->hash.cofac[0] == 1;
+}
 // lines of the Miller walk of types f, d, g: one tangent per loop position, one chord per non-zero digit
 // strictly between the top digit and digit 0 (miller_cc_walk)
 static size_t cc_table_rows_compute(const pbc_b200_pairing_s* p) {
   BigUInt r;
   if (p->dwide) for (int i = pbcb200_dw::kLimbs; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->dw_cc.r[i]);
   else for (int i = kNS; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->cc.r[i]);
-  std::vector<int8_t> dg = naf_digits(r);
+  std::vector<int8_t> dg = miller_naf_digits(r, g1_cofactor_one(p));
   size_t rows = dg.size() - 1;
   for (size_t m = 1; m + 1 < dg.size(); m++) rows += dg[m] ? 1 : 0;
   return rows;
@@ -381,7 +387,7 @@ static int init_type_a1(pbc_b200_pairing_s* p, const std::map<std::string, std::
   gc.zlen = p->zr.zlen;
   gc.count = (uint32_t)wb;
   {
-    std::vector<int8_t> dg = naf_digits(n);
+    std::vector<int8_t> dg = miller_naf_digits(n, false);       // E(F_p) has order l n, l > 1
     if (dg.size() > 32 * (size_t)kMaxLimbs) return fail("type a1: n too large for the signed-digit table");
     memset(&p->a1naf, 0, sizeof p->a1naf);
     for (size_t i = 0; i < dg.size(); i++) {
@@ -765,7 +771,7 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
     p->derived["sqrt_nonresidue"] = {z};
   }
   {
-    std::vector<int8_t> dg = naf_digits(r);
+    std::vector<int8_t> dg = miller_naf_digits(r, g1_cofactor_one(p));
     memset(&p->dw_naf, 0, sizeof p->dw_naf);
     for (size_t i = 0; i < dg.size(); i++) {
       if (dg[i]) p->dw_naf.nz[i >> 5] |= 1u << (i & 31);
@@ -1132,10 +1138,10 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
     CUDA_OK(cudaMemcpyToSymbol(c_hash, &p->hash, sizeof(HashConsts)));
     if (p->type == 'f' || p->type == 'd' || p->type == 'g') CUDA_OK(cudaMemcpyToSymbol(c_cc, &p->cc, sizeof(CCConsts)));
     if (p->type == 'f' || p->type == 'd' || p->type == 'g') {
-      // signed digits of the group order (host_naf.hpp); r is what fill_cc stored
+      // signed digits of the Miller walk (miller_naf_digits, host_naf.hpp); r is what fill_cc stored
       BigUInt r;
       for (int i = kNS; i-- > 0;) r = r.shl(32) + BigUInt((uint64_t)p->cc.r[i]);
-      std::vector<int8_t> dg = naf_digits(r);
+      std::vector<int8_t> dg = miller_naf_digits(r, g1_cofactor_one(p));
       memset(&p->ccnaf, 0, sizeof p->ccnaf);
       for (size_t i = 0; i < dg.size() && i < 256; i++) {
         if (dg[i]) p->ccnaf.nz[i >> 5] |= 1u << (i & 31);

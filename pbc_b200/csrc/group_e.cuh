@@ -75,6 +75,9 @@ k_e_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   uint32_t x[kNA1], one[kNA1] = {1};
   O::set_const(sT, c_fp.r2);
   a1_limbs_from_be(x, G + idx * (size_t)wb, wb);
+  uint32_t nz = 0;
+#pragma unroll
+  for (int i = 0; i < kNA1; i++) nz |= x[i];
   O::st(sB, x);
   O::mul(sB, sT, sB);
   uint32_t k[kNA1];
@@ -88,7 +91,8 @@ k_e_gt_pow(const uint8_t* __restrict__ G, const uint8_t* __restrict__ K, uint8_t
   O::st(sT, one);
   O::mul(sA, sA, sT);              // leave Montgomery form
   O::ld(x, sA);
-  if (top < 0) {                   // k = 0: the identity
+  if (top < 0 && nz) {             // k = 0: the identity, except for a zero base: fp_pow_mpz
+                                   // (arith/montfp.c:379-396) leaves 0 at 0 whatever the exponent
 #pragma unroll
     for (int i = 0; i < kNA1; i++) x[i] = one[i];
   }

@@ -34,4 +34,17 @@ inline std::vector<int8_t> naf_digits(const BigUInt& n) {
   return d;
 }
 
+// The digits the Miller loops walk for a group order r (odd).  The reference scans the bits of r from
+// the second highest down to bit 1 and ends on a tangent, so it evaluates f_{r-1,P}.  A signed scan of
+// r itself ends on the tangent at (r + 1)/2 P where r = 3 mod 4, i.e. evaluates f_{r+1,P}; the two
+// differ by the lines through P and (r - 1) P, r P, which are vertical (killed by the final
+// exponentiation) only when r P = O.  So where the curve has points outside E[r] (cofactor > 1) the
+// walk takes the digits of r - 1: digit 0 is 0 and never read, the others are the non-adjacent form of
+// (r - 1)/2, and the walk gives f_{r-1,P} for every P on the curve.  Where r = 1 mod 4 these are the
+// digits of r with digit 0 cleared, the same walk.  With cofactor 1 every point has r P = O and the
+// digits of r are kept (for g149 they have one chord fewer).
+inline std::vector<int8_t> miller_naf_digits(const BigUInt& r, bool cofactor_one) {
+  return cofactor_one ? naf_digits(r) : naf_digits(r - BigUInt(1));
+}
+
 }  // namespace pbcb200

@@ -35,11 +35,11 @@ struct CCConstsT {
 typedef CCConstsT<kNS> CCConsts;
 __constant__ CCConsts c_cc;
 
-// The loop scans the non-adjacent form of r (host_naf.hpp) instead of its bits: one chord + addition
-// per three positions instead of one per two; where the digit is -1 the chord goes through V and -P.
-// Vertical lines and constants lie in the subfield the final exponentiation kills, so the reduced
-// pairing is the same element (the reference keeps the plain scan).  Faster for F, D and G (fewer
-// chord steps).
+// The loop scans signed digits (miller_naf_digits, host_naf.hpp: the non-adjacent form of r - 1, or of
+// r where the cofactor is 1) instead of the bits of r: one chord + addition per three positions instead
+// of one per two; where the digit is -1 the chord goes through V and -P.  Vertical lines and constants
+// lie in the subfield the final exponentiation kills, so the reduced pairing is the same element for
+// every P on the curve (the reference keeps the plain scan).  Faster for F, D and G (fewer chord steps).
 struct CCNaf {
   uint32_t nz[8], neg[8];      // bit i: digit i non-zero / digit i is -1   (r below 2^255)
   uint32_t len;                // number of digits; the top one is +1

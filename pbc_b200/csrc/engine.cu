@@ -1198,6 +1198,38 @@ static size_t inv_threads(const pbc_b200_pairing_s* p, size_t n, size_t per_sm) 
 }
 
 // ------------------------------------------------------------------------------------------
+// the final stage of types a, a1 and e on n Miller values in the limb-major Montgomery layout the
+// Miller kernels write: batch inversion of dprod in place (prefix: scratch of its shape), then the
+// final exponentiation into d_out (GT wire format).  The one launch path of these stages: the pairings
+// (enqueue_pairings) and the test hook (pbc_b200_tower_op op 3) both come here.
+// ------------------------------------------------------------------------------------------
+static int enqueue_final(pbc_b200_pairing_s* p, void* f, void* dprod, void* prefix, uint8_t* d_out, size_t n,
+                         cudaStream_t st, cudaEvent_t* ev) {
+  if (p->type == 'a') {
+    size_t T = inv_threads(p, n, 256);
+    unsigned gi = (unsigned)((T + kBlockInv - 1) / kBlockInv);
+    k_batch_invert<kNA, true, kBlockInv><<<gi, kBlockInv, kSmemInv16, st>>>(dprod, prefix, n, T);
+    LAUNCHED();
+    if (ev) cudaEventRecord(ev[2], st);
+    unsigned gf = (unsigned)((n + kBlockFinal - 1) / kBlockFinal);
+    k_a_finalexp<kBlockFinal><<<gf, kBlockFinal, kSmemAFinal, st>>>((const uint4*)f, (const uint4*)dprod, d_out, n);
+    LAUNCHED();
+    return 0;
+  }
+  if (p->type != '1' && p->type != 'e') return fail("pairing type '%c' has no batched final stage", p->type);
+  size_t T = inv_threads(p, n, 128);
+  unsigned gi = (unsigned)((T + kBlockA1Small - 1) / kBlockA1Small);
+  k_batch_invert<kNA1, false, kBlockA1Small><<<gi, kBlockA1Small, kSmemInv34, st>>>(dprod, prefix, n, T);
+  LAUNCHED();
+  if (ev) cudaEventRecord(ev[2], st);
+  unsigned gf = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
+  if (p->type == '1') k_a1_finalexp<kBlockA1Small><<<gf, kBlockA1Small, kSmemA1Final, st>>>(f, dprod, d_out, n);
+  else k_e_finalexp<kBlockA1Small><<<gf, kBlockA1Small, kSmemEFinal, st>>>(f, dprod, d_out, n);
+  LAUNCHED();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
 // enqueue one batch of n_out outputs of `job`, device buffers, on `st`.  ws: ws_bytes() bytes.
 // ------------------------------------------------------------------------------------------
 static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_out, const uint8_t* d_in1,
@@ -1245,14 +1277,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       LAUNCHED();
     }
     STAGE(1);
-    size_t T = inv_threads(p, n, 128);
-    unsigned gi = (unsigned)((T + kBlockA1Small - 1) / kBlockA1Small);
-    k_batch_invert<kNA1, false, kBlockA1Small><<<gi, kBlockA1Small, kSmemInv34, st>>>(dprod, prefix, n, T);
-    LAUNCHED();
-    STAGE(2);
-    unsigned gf = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
-    k_a1_finalexp<kBlockA1Small><<<gf, kBlockA1Small, kSmemA1Final, st>>>(f, dprod, d_out, n);
-    LAUNCHED();
+    if (enqueue_final(p, f, dprod, prefix, d_out, n, st, ev)) return 1;
     STAGE(3);
     CUDA_OK(cudaGetLastError());
     return 0;
@@ -1298,14 +1323,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       LAUNCHED();
     }
     STAGE(1);
-    size_t T = inv_threads(p, n, 128);
-    unsigned gi = (unsigned)((T + kBlockA1Small - 1) / kBlockA1Small);
-    k_batch_invert<kNA1, false, kBlockA1Small><<<gi, kBlockA1Small, kSmemInv34, st>>>(dprod, prefix, n, T);
-    LAUNCHED();
-    STAGE(2);
-    unsigned gf = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
-    k_e_finalexp<kBlockA1Small><<<gf, kBlockA1Small, kSmemEFinal, st>>>(f, dprod, d_out, n);
-    LAUNCHED();
+    if (enqueue_final(p, f, dprod, prefix, d_out, n, st, ev)) return 1;
     STAGE(3);
     CUDA_OK(cudaGetLastError());
     return 0;
@@ -1365,14 +1383,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       LAUNCHED();
     }
     STAGE(1);
-    size_t T = inv_threads(p, n, 256);
-    unsigned gi = (unsigned)((T + kBlockInv - 1) / kBlockInv);
-    k_batch_invert<kNA, true, kBlockInv><<<gi, kBlockInv, kSmemInv16, st>>>(dprod, prefix, n, T);
-    LAUNCHED();
-    STAGE(2);
-    unsigned gf = (unsigned)((n + kBlockFinal - 1) / kBlockFinal);
-    k_a_finalexp<kBlockFinal><<<gf, kBlockFinal, kSmemAFinal, st>>>(f, dprod, d_out, n);
-    LAUNCHED();
+    if (enqueue_final(p, f, dprod, prefix, d_out, n, st, ev)) return 1;
     STAGE(3);
     CUDA_OK(cudaGetLastError());
     return 0;
@@ -2395,6 +2406,62 @@ __global__ void k_fq_op(int op, uint8_t* __restrict__ out, const uint8_t* __rest
   fq_to_wire_w<W>(out + idx * W, x);
 }
 
+// ---- tower_op 3 for types a, a1 and e: GT wire elements -> the Miller-value layout of the final stage ----
+// Element e of a limb-major batch array, as Ops::st_global writes it: vector v (VW words) at (e * N / VW + v) * n + idx.
+template <int N, int VW>
+__device__ __forceinline__ void mv_store(void* g, int e, size_t n, size_t idx, const uint32_t* x) {
+  uint32_t* w = reinterpret_cast<uint32_t*>(g);
+#pragma unroll
+  for (int v = 0; v < N / VW; v++)
+#pragma unroll
+    for (int k = 0; k < VW; k++) w[(((size_t)e * (N / VW) + v) * n + idx) * VW + k] = x[v * VW + k];
+}
+// wire coordinate (wb bytes, big-endian, any value below 2^(8 wb)) -> Montgomery form, reduced mod q as
+// element_from_bytes reduces it.  R^2 is the full operand and the wire value the scanned one (a1_load_point).
+template <int N, bool FULL>
+__device__ __forceinline__ void mv_coord(uint32_t* x, const uint8_t* p, int wb) {
+  uint32_t w[N];
+  if constexpr (N == kNA) limbs_from_be<kNA, kWA>(w, p);
+  else a1_limbs_from_be(w, p, wb);
+  mont_mul<N, FULL>(x, c_fp.r2, w);
+}
+// types a and a1: f = (x, y) from an F_q^2 element x || y, and D = N(f) f0 f1 = (f0^2 + f1^2) f0 f1 as the
+// Miller kernels publish it (a_publish, a1_publish): 0 exactly when f0 f1 = 0, the final stage's shortcut to 1.
+template <int N, bool FULL, int VW>
+__global__ void k_a_mv_from_wire(void* __restrict__ f, void* __restrict__ dprod, const uint8_t* __restrict__ in,
+                                 size_t n, int wb) {
+  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  uint32_t f0[N], f1[N], s[N], t[N];
+  mv_coord<N, FULL>(f0, in + idx * 2 * (size_t)wb, wb);
+  mv_coord<N, FULL>(f1, in + idx * 2 * (size_t)wb + wb, wb);
+  mv_store<N, VW>(f, 0, n, idx, f0);
+  mv_store<N, VW>(f, 1, n, idx, f1);
+  mont_mul<N, FULL>(s, f0, f0);
+  mont_mul<N, FULL>(t, f1, f1);
+  fp_add<N, FULL>(s, s, t);
+  mont_mul<N, FULL>(t, f0, f1);
+  mont_mul<N, FULL>(s, s, t);
+  mv_store<N, VW>(dprod, 0, n, idx, s);
+}
+// type e: f = v from a, dprod = vd from b (e_publish), b == nullptr: vd = 1
+__global__ void k_e_mv_from_wire(void* __restrict__ f, void* __restrict__ dprod, const uint8_t* __restrict__ a,
+                                 const uint8_t* __restrict__ b, size_t n) {
+  size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const int wb = (int)c_a1.wb;
+  uint32_t x[kNA1];
+  mv_coord<kNA1, false>(x, a + idx * (size_t)wb, wb);
+  mv_store<kNA1, 2>(f, 0, n, idx, x);
+  if (b) {
+    mv_coord<kNA1, false>(x, b + idx * (size_t)wb, wb);
+  } else {
+#pragma unroll
+    for (int k = 0; k < kNA1; k++) x[k] = c_fp.one[k];
+  }
+  mv_store<kNA1, 2>(dprod, 0, n, idx, x);
+}
+
 // element_cmp on wire bytes (canonical residues: equal elements <=> equal bytes): flags[i] = 1 if a[i] != b[i]
 __global__ void k_bytes_cmp(uint8_t* __restrict__ flags, const uint8_t* __restrict__ a, const uint8_t* __restrict__ b,
                             size_t len, size_t n) {
@@ -2475,18 +2542,50 @@ extern "C" int pbc_b200_fp_op(pbc_b200_pairing_t* p, int op, unsigned char* out,
   return 0;
 }
 
-/* GT-sized differential-test hook for the extension towers of types f and d (see k_f_tower_op,
- * k_d_tower_op): operands and results in GT wire format. */
+/* GT-sized differential-test hook for the extension towers of types f, d and g (see k_f_tower_op,
+ * k_d_tower_op, k_g_tower_op) and for the final stage of types a, a1 and e (op 3: enqueue_final on
+ * Miller values made by k_a_mv_from_wire / k_e_mv_from_wire): operands and results in GT wire format. */
 extern "C" int pbc_b200_tower_op(pbc_b200_pairing_t* p, int op, unsigned char* out,
                                  const unsigned char* a, const unsigned char* b, size_t n) {
-  if (!p) return fail("null argument");
-  if (p->type != 'f' && p->type != 'd' && p->type != 'g') return fail("tower_op: types f, d and g only");
+  if (!p || (n && (!out || !a))) return fail("null argument");
+  const bool batched_final = p->type == 'a' || p->type == '1' || p->type == 'e';
+  if (!batched_final && p->type != 'f' && p->type != 'd' && p->type != 'g') return fail("tower_op: types a, a1, e, f, d and g only");
+  if (batched_final && op != 3) return fail("tower_op: types a, a1 and e have op 3 only");
   if (n == 0) return 0;
   int dev = 0;
   CUDA_OK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> dev_lock(g_dev_mu[dev & 63]);
   if (ctx_prepare(p, dev)) return 1;
   size_t wb = (size_t)p->gt_len;
   DevBuf da, db, dout;
+  if (batched_final) {
+    // the final stage every pairing of these types takes (enqueue_final), on the caller's elements: they go
+    // into the Miller-value layout first -- f and D = N(f) f0 f1 (a, a1), v and vd (e)
+    const size_t el = p->type == 'a' ? (size_t)kNA * 4 : (size_t)kNA1 * 4;   // bytes per F_q element
+    const size_t fw = p->type == 'e' ? 1 : 2;                                 // F_q elements per Miller value
+    DevBuf ws;
+    CUDA_OK(ws.alloc(n * el * (fw + 2)));
+    uint8_t* f = ws.as<uint8_t>();
+    uint8_t* dprod = f + fw * el * n;
+    uint8_t* prefix = dprod + el * n;
+    if (p->type == 'e' && b) {
+      CUDA_OK(db.alloc(n * wb));
+      CUDA_OK(cudaMemcpy(db.p, b, n * wb, cudaMemcpyHostToDevice));
+    }
+    CUDA_OK(da.alloc(n * wb));
+    CUDA_OK(dout.alloc(n * wb));
+    CUDA_OK(cudaMemcpy(da.p, a, n * wb, cudaMemcpyHostToDevice));
+    unsigned g = (unsigned)((n + 127) / 128);
+    if (p->type == 'a') k_a_mv_from_wire<kNA, true, 4><<<g, 128>>>(f, dprod, da.as<uint8_t>(), n, kWA);
+    else if (p->type == '1') k_a_mv_from_wire<kNA1, false, 2><<<g, 128>>>(f, dprod, da.as<uint8_t>(), n, (int)(wb / 2));
+    else k_e_mv_from_wire<<<g, 128>>>(f, dprod, da.as<uint8_t>(), db.as<uint8_t>(), n);
+    LAUNCHED();
+    if (enqueue_final(p, f, dprod, prefix, dout.as<uint8_t>(), n, 0, nullptr)) return 1;
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaDeviceSynchronize());
+    CUDA_OK(cudaMemcpy(out, dout.p, n * wb, cudaMemcpyDeviceToHost));
+    return 0;
+  }
   CUDA_OK(da.alloc(n * wb));
   CUDA_OK(db.alloc(n * wb));
   CUDA_OK(dout.alloc(n * wb));

@@ -264,6 +264,10 @@ class Pairing:
         return out.raw[:n * wb * widths[2]]
 
     def tower_op(self, op: int, a: bytes, b, n: int) -> bytes:
+        """pbc_b200_tower_op: n GT wire elements in a (and b), n out.  Types f, d, g: the extension-tower
+        ops 0-6.  Types a, a1, e: op 3 only, the final stage the pairings run (batch inversion, then the
+        final exponentiation) on Miller values given in GT wire format -- a, a1: f = a[i], f0 f1 = 0 gives
+        1; e: numerator a[i] over denominator b[i] (1 where b is None), vd = 0 gives 1, v = 0 gives 0."""
         out = C.create_string_buffer(n * self.gt_len)
         if lib.pbc_b200_tower_op(self._h, op, C.addressof(out), _addr(a), _addr(b), n):
             raise PairingError(last_error())

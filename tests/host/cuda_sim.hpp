@@ -101,4 +101,10 @@ static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess
 static inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t, cudaEvent_t) { *ms = 0; return cudaSuccess; }
 template <class K> static inline cudaError_t cudaFuncSetAttribute(K, int, int) { return cudaSuccess; }
 enum { cudaDevAttrMultiProcessorCount = 16 };
-static inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 132; return cudaSuccess; }   // an H100 SXM's multiprocessors
+// an H100 SXM's 132 multiprocessors; PBC_SIM_SMS=N reports N, so that a small batch spans several
+// batch-inversion chains per thread (T = multiprocessors * 128 or 256 chains, engine.cu inv_threads)
+static inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) {
+  const char* e = getenv("PBC_SIM_SMS");
+  *v = e && atoi(e) > 0 ? atoi(e) : 132;
+  return cudaSuccess;
+}

@@ -77,6 +77,26 @@ def test_gpu_parity_tests_pass_on_the_simulator(sim):
     assert passed >= 310, tail
 
 
+def test_final_exponentiation_file_on_the_simulator(sim):
+    """tests/test_gpu_final_exponentiation.py at reduced sizes.  The simulator reports one multiprocessor
+    (PBC_SIM_SMS=1), so its batch-inversion chains are four elements long, as they are on a GPU for the
+    file's batches of a little over three times the chain count"""
+    env = _env(sim)
+    env["PBC_FINAL_EXP_REDUCED"] = "1"
+    env["PBC_SIM_SMS"] = "1"
+    cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
+           os.path.join(ROOT, "tests", "test_gpu_final_exponentiation.py")]
+    try:
+        import xdist  # noqa: F401
+        cmd += ["-n", str(max(1, min(8, len(os.sched_getaffinity(0)))))]
+    except Exception:
+        pass
+    out = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=3000, cwd=ROOT)
+    assert out.returncode == 0, out.stdout[-3000:]
+    tail = out.stdout.strip().splitlines()[-1]
+    assert int(tail.split(" passed")[0].split()[-1]) >= 15, tail
+
+
 def test_multiplier_work_counted_by_the_simulator_matches_bench(sim):
     """bench.py's roofline numerator (32x32 products the Miller kernel executes per pairing) against
     the count the PTX interpreter takes while running that kernel"""

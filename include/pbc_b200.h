@@ -32,12 +32,31 @@
  *     pairings ANY infinite input makes the whole product 1 (element_prod_pairing, :153-171);
  *   - powers in G1 and G2 are the exact k P (k reduced mod r, mod n for type a1) for any point P on
  *     the curve, including points of small order and type a1's subgroup elements of order p1 or p2;
- *   - every output is bit-identical to the reference CPU path.
+ *   - every output is bit-identical to the reference CPU path, including first and second arguments
+ *     of small order (points of E(F_q) outside G1, twist points outside G2), second arguments drawn
+ *     on the twist without cofactor multiplication, and twist points with y = 0 (types d, g: x a
+ *     root of x^3 + a x + b) -- wherever the reference's own computation does not divide by zero.
  * One input is DEFINED here rather than copied: a first or second argument with y = 0 (type a, a1: the
  * 2-torsion point (0, 0); types d, g: a 2-torsion point of E(F_q) if the cofactor is even) lies on the
  * curve but outside the order-r groups and has no tangent line; the reference's projective doubling
  * inverts Z = 0 there and returns a by-product of that.  This library decodes such a point as the
  * point at infinity: the pairing is 1 (tests/test_gpu_edge_cases.py).
+ * The other inputs on which the reference divides by zero (tests/test_gpu_small_order_pairings.py):
+ *   - type a, a first argument of small order whose walk reaches O (the reference inverts Z = 0 in
+ *     point_to_affine and goes on from the by-product) or whose last chord joins V to itself (the
+ *     Miller value is 0 and the final exponentiation inverts it): the pairing is 1, and a product of
+ *     pairings containing such a pair is 1, as for a Miller value with f0 f1 = 0;
+ *   - type g, a pair whose Miller value lies in F_q^5 (a twist point of small order as the second
+ *     argument, for one): the reference's Lucas step divides by P^2 - 4 = 0 and exits; the pairing is
+ *     1, its exact value, and in a product the pair contributes 1;
+ *   - types f, d, g, a first argument of small order whose walk reaches O: the reference's affine walk
+ *     goes on from the stale coordinates of O and its final exponentiation inverts 0 and exits.  Here
+ *     the next addition of +-P turns the Jacobian O into (0, 0, 0), after which every line is 0 (or a
+ *     chord joins V to itself, which is 0 as well), so the Miller value is 0 and the output is the
+ *     ZERO of F_q^k (all-zero bytes), which is not an element of GT: for the
+ *     pairing, for pp one-shot and through a handle, and for every product holding such a pair (unless
+ *     another input of that product is O, which makes it 1).  A caller that needs a GT element must
+ *     keep such points out, e.g. by checking r P = O.
  * Type E (k = 1): e(P, Q) is bit-exact for P and Q in G1 (points of order r).  The Miller loop
  * evaluates at Q + R and at R, R a point outside E[r] that the library fixes at init
  * (pbc_b200_derived_constant "R", x then y); the reference draws its R at random per pairing_init.

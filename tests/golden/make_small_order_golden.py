@@ -33,6 +33,7 @@ sys.path.insert(0, ROOT)
 from oracle import ref as R  # noqa: E402
 from oracle import pbc_oracle as O  # noqa: E402
 from pbc_b200.params import PARAMS  # noqa: E402
+from tests.small_order_points import random_point  # noqa: E402
 
 SEED = 20261016
 SMALL_P = 100           # primes below this count as small factors
@@ -51,62 +52,6 @@ def small_factors(N, bound):
 
 def primes_of(m):
     return [p for p in range(2, m + 1) if m % p == 0 and all(p % d for d in range(2, p))]
-
-
-def kpow(K, a, e):
-    r = K.one
-    for bit in bin(e)[2:]:
-        r = K.sqr(r)
-        if bit == "1":
-            r = K.mul(r, a)
-    return r
-
-
-def rand_el(K, rnd):
-    if isinstance(K, O.PrimeField):
-        return rnd.randrange(K.p)
-    if isinstance(K, O.QuadExt):
-        return (rand_el(K.b, rnd), rand_el(K.b, rnd))
-    return tuple(rand_el(K.b, rnd) for _ in range(K.n))
-
-
-def sqrt_el(K, a, size, rnd):
-    """Tonelli-Shanks in a field of `size` elements; None if a is not a square"""
-    if K.eq(a, K.zero):
-        return a
-    if not K.eq(kpow(K, a, (size - 1) // 2), K.one):
-        return None
-    s, t = 0, size - 1
-    while t % 2 == 0:
-        t //= 2
-        s += 1
-    minus1 = K.neg(K.one)
-    while True:
-        z = rand_el(K, rnd)
-        if K.eq(kpow(K, z, (size - 1) // 2), minus1):
-            break
-    c, x, b, m = kpow(K, z, t), kpow(K, a, (t + 1) // 2), kpow(K, a, t), s
-    while not K.eq(b, K.one):
-        i, b2 = 0, b
-        while not K.eq(b2, K.one):
-            b2 = K.sqr(b2)
-            i += 1
-        g = c
-        for _ in range(m - i - 1):
-            g = K.sqr(g)
-        x, c = K.mul(x, g), K.sqr(g)
-        b, m = K.mul(b, c), i
-    return x
-
-
-def random_point(E, size, rnd):
-    K = E.K
-    while True:
-        x = rand_el(K, rnd)
-        rhs = K.add(K.mul(K.add(K.sqr(x), E.a), x), E.b)
-        y = sqrt_el(K, rhs, size, rnd)
-        if y is not None and not K.eq(y, K.zero):
-            return (x, y)
 
 
 def trace_power(t, q, k):

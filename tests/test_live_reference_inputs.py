@@ -198,7 +198,7 @@ def _sim(tmp, script):
     return so
 
 
-def _run_gpu_file(so, selection, min_passed):
+def _run_gpu_file(so, selection, min_passed, name="test_gpu_live_reference.py"):
     if not os.path.exists(L.REF_LIB):
         pytest.skip(L.ref_missing_message())
     env = dict(os.environ)
@@ -207,7 +207,7 @@ def _run_gpu_file(so, selection, min_passed):
     env["PYTHONPATH"] = ROOT + os.pathsep + env.get("PYTHONPATH", "")
     # the _device forms take torch.cuda tensors: without a CUDA device the reduced run leaves them out
     cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider"]
-    cmd += ["-k", selection, os.path.join(ROOT, "tests", "test_gpu_live_reference.py")]
+    cmd += ["-k", selection, os.path.join(ROOT, "tests", name)]
     try:
         import xdist  # noqa: F401
         cmd += ["-n", str(max(1, min(8, len(os.sched_getaffinity(0)))))]
@@ -231,3 +231,14 @@ def test_live_reference_file_on_the_eight_limb_simulator(tmp_path):
     sel = " or ".join("%s_set" % s for s in L.WIDE_D)
     sel += " or (outside_g1 and (%s))" % " or ".join(s for s in L.WIDE_D if s != "d224")
     _run_gpu_file(so, sel, 40)
+
+
+def test_small_order_pairings_file_on_the_simulator(tmp_path):
+    so = _sim(tmp_path, "make_host_sim.py")
+    sel = " or ".join("%s_set" % s for s in ("a", "d159", "g149", "f")) + " or sharing"
+    _run_gpu_file(so, sel, 18, "test_gpu_small_order_pairings.py")
+
+
+def test_small_order_pairings_file_on_the_eight_limb_simulator(tmp_path):
+    so = _sim(tmp_path, "make_host_sim_d_wide.py")
+    _run_gpu_file(so, "d190_set or d201_set", 8, "test_gpu_small_order_pairings.py")

@@ -133,6 +133,25 @@ int pbc_b200_prod_pairings_apply(pbc_b200_pairing_t *p, unsigned char *out,
 int pbc_b200_prod_pairings_apply_device(pbc_b200_pairing_t *p, void *d_out, const void *d_in1,
                                         const void *d_in2, size_t k, size_t n_out, void *stream);
 
+/* Batched element_prod_pairing with a pair count per output (ragged batches, e.g. aggregate
+ * signatures over different numbers of messages):
+ *   out[i] = prod_{offsets[i] <= j < offsets[i+1]} e(in1[j], in2[j]),   i < n_out.
+ * Each output is byte-identical to pbc_b200_prod_pairings_apply(k = its length, n_out = 1) on its
+ * pairs, with the same rules (an O or off-curve input makes that output 1, and only that output).
+ * offsets: n_out + 1 entries in HOST memory for both forms, offsets[0] = 0, strictly increasing (an
+ * empty product is rejected, as k = 0 is above); the library has read them by the time the call
+ * returns.  NULL offsets, offsets[0] != 0, a non-increasing entry (the message names its index) and a
+ * byte count that overflows size_t fail before any CUDA call; n_out = 0 returns 0 and touches nothing.
+ * Every pair runs its own Miller loop; the Miller values of each output are multiplied in passes of at
+ * most 16 consecutive values per thread, so one long product costs log16(length) passes, not one
+ * thread's serial loop.  The host form cuts the batch into chunks of whole outputs (multi-GPU: slices
+ * of whole outputs balanced by pairs); the device form is asynchronous on `stream`, its workspace grows
+ * to the largest call. */
+int pbc_b200_prod_pairings_apply_v(pbc_b200_pairing_t *p, unsigned char *out, const unsigned char *in1,
+                                   const unsigned char *in2, const size_t *offsets, size_t n_out);
+int pbc_b200_prod_pairings_apply_v_device(pbc_b200_pairing_t *p, void *d_out, const void *d_in1,
+                                          const void *d_in2, const size_t *offsets, size_t n_out, void *stream);
+
 /* Batched pairing_pp_init + pairing_pp_apply (include/pbc_pairing.h:54-89,
  * ecc/a_param.c:149-220,317-360): one fixed first argument, n second arguments.
  *   out[i] = e(in1, in2[i]). */

@@ -35,6 +35,8 @@ lib.pbc_b200_pairings_apply.argtypes = [_P, _P, _P, _P, C.c_size_t]
 lib.pbc_b200_pairings_apply_device.argtypes = [_P, _P, _P, _P, C.c_size_t, _P]
 lib.pbc_b200_prod_pairings_apply.argtypes = [_P, _P, _P, _P, C.c_size_t, C.c_size_t]
 lib.pbc_b200_prod_pairings_apply_device.argtypes = [_P, _P, _P, _P, C.c_size_t, C.c_size_t, _P]
+lib.pbc_b200_prod_pairings_apply_v.argtypes = [_P, _P, _P, _P, _P, C.c_size_t]
+lib.pbc_b200_prod_pairings_apply_v_device.argtypes = [_P, _P, _P, _P, _P, C.c_size_t, _P]
 lib.pbc_b200_pp_pairings_apply.argtypes = [_P, _P, _P, _P, C.c_size_t]
 lib.pbc_b200_pp_pairings_apply_device.argtypes = [_P, _P, _P, _P, C.c_size_t, _P]
 lib.pbc_b200_pp_init.argtypes = [_P, C.POINTER(_P), _P]

@@ -7,9 +7,11 @@
 // runs on the GPU.
 #include <cuda_runtime.h>
 #include <stdarg.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <map>
 #include <mutex>
@@ -44,6 +46,7 @@ namespace pbcb200_dw {
 int dw_upload(const DWideConsts&) { return -2; }
 void dw_miller(const uint8_t*, const uint8_t*, uint32_t*, uint32_t*, size_t, size_t, const uint32_t*, size_t, cudaStream_t) {}
 void dw_prod(const uint32_t*, const uint32_t*, uint32_t*, uint32_t*, size_t, size_t, size_t, cudaStream_t) {}
+void dw_prod_v(const uint32_t*, const uint32_t*, size_t, uint32_t*, uint32_t*, size_t, const uint64_t*, size_t, cudaStream_t) {}
 void dw_finalexp(const uint32_t*, const uint32_t*, uint8_t*, size_t, cudaStream_t) {}
 void dw_pp_init(const uint8_t*, uint32_t*, size_t, cudaStream_t) {}
 void dw_group(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
@@ -140,6 +143,14 @@ struct DevCtx {
   bool ws_used = false;
   // optional per-stage timing of the device-API path (bench.py roofline)
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  // pinned staging of the run tables of pbc_b200_prod_pairings_apply_v (upload_plan): a call copies its
+  // table here and enqueues the upload, so it returns without waiting for the stream and never reads
+  // the caller's offsets afterwards.  Slots are reused round robin once their last upload has run.
+  static constexpr int kPlanSlots = 4;
+  uint64_t* plan_h[kPlanSlots] = {};
+  size_t plan_cap[kPlanSlots] = {};    // bytes
+  cudaEvent_t plan_ev[kPlanSlots] = {};
+  int plan_next = 0;
 };
 
 struct pbc_b200_pairing_s {
@@ -203,11 +214,46 @@ static constexpr int kBlockInv = 128;
 static constexpr int kBlockCC = 128;           // types f, d: threads per block
 static constexpr int kBlockCCMiller = kCCMillerBlock;   // ... of the Miller kernels (lock-step barrier)
 
-// The three reference operations that reach the GPU (include/pbc_pairing.h:141-171, :54-89).
-enum Mode { kSingle = 0, kProd = 1, kPP = 2 };
+// pbc_b200_prod_pairings_apply_v: the passes of the segmented product (prod_v.cuh) for one batch,
+// built on the host from the offsets.  Pass s has count[s] runs of at most kProdVRun consecutive values
+// of one output; the last pass has one run per output.
+struct ProdPlan {
+  size_t pairs = 0;            // Miller values of the batch
+  size_t part = 0;             // elements of each of the two partial-product buffers (0: one pass)
+  std::vector<size_t> count;   // runs per pass
+  std::vector<uint64_t> runs;  // per pass, count + 1 input indices: run r is [runs[r], runs[r + 1])
+};
+// off: n_out + 1 increasing entries, rebased here to off[0] = 0
+static ProdPlan prod_plan(const size_t* off, size_t n_out) {
+  ProdPlan pl;
+  pl.pairs = off[n_out] - off[0];
+  std::vector<uint64_t> cur(n_out + 1), next(n_out + 1);
+  for (size_t i = 0; i <= n_out; i++) cur[i] = off[i] - off[0];
+  for (;;) {
+    bool last = true;
+    size_t runs = 0;
+    next[0] = 0;
+    for (size_t i = 0; i < n_out; i++) {
+      for (uint64_t j = cur[i]; j < cur[i + 1]; j += kProdVRun, runs++) pl.runs.push_back(j);
+      if (cur[i + 1] - cur[i] > (uint64_t)kProdVRun) last = false;
+      next[i + 1] = runs;
+    }
+    pl.runs.push_back(cur[n_out]);
+    pl.count.push_back(runs);
+    if (last) break;
+    if (pl.count.size() == 1) pl.part = runs;    // the largest partial batch: later passes only shrink
+    cur.swap(next);
+  }
+  return pl;
+}
+
+// The three reference operations that reach the GPU (include/pbc_pairing.h:141-171, :54-89), and
+// element_prod_pairing with a pair count per output (kProdV).
+enum Mode { kSingle = 0, kProd = 1, kPP = 2, kProdV = 3 };
 struct Job {
   Mode mode = kSingle;
   size_t k = 1;                // kProd: pairings per output
+  const ProdPlan* plan = nullptr;   // kProdV: pairs and passes
   // kPP through a pairing_pp_t (pbc_b200_pp_init): what the handle keeps on the device -- the
   // line-coefficient table (types a, a1) and the wire bytes of the fixed first argument (all types).
   // nullptr: the table is built inside the call (pbc_b200_pp_pairings_apply).
@@ -219,13 +265,41 @@ static size_t cc_table_bytes(const pbc_b200_pairing_s* p);
 // type e: the fixed-argument table (pairing_e.cuh, e_pp_rows) and its flag word
 static size_t e_table_bytes(const pbc_b200_pairing_s* p) { return (e_pp_rows(p->e.exp2) * kNA1 + 4) * 4; }
 
+// kProdV: bytes of the value of one partial product of the segmented product, and of its validity
+static size_t prodv_value_bytes(const pbc_b200_pairing_s* p) {
+  if (p->type == 'a') return 2 * 64;                        // f [2]
+  if (p->type == '1') return 2 * (size_t)kNA1 * 4;          // f [2]
+  if (p->type == 'e') return (size_t)kNA1 * 4;              // v
+  const size_t W = p->type == 'f' ? kF12Words : (p->type == 'g' ? kF10Words : 6 * (size_t)p->nlimbs);
+  return W * 4;
+}
+static size_t prodv_valid_bytes(const pbc_b200_pairing_s* p) {
+  if (p->type == 'a') return 64;                            // d
+  if (p->type == '1' || p->type == 'e') return (size_t)kNA1 * 4;   // d, vd
+  return 4;                                                 // flag word
+}
+static size_t prodv_elem_bytes(const pbc_b200_pairing_s* p) { return prodv_value_bytes(p) + prodv_valid_bytes(p); }
+static size_t round16(size_t b) { return (b + 15) & ~(size_t)15; }
+static size_t ws_core(const pbc_b200_pairing_s* p, const Job& job, size_t n_out);
+// kProdV: the run tables and the two partial-product buffers follow everything the uniform product
+// lays out for the same Miller values (ws_core), the type F slot kernels' scratch included
+static size_t prodv_tail_off(const pbc_b200_pairing_s* p, const Job& job, size_t n_out) {
+  return round16(ws_core(p, job, n_out));
+}
 // workspace bytes for n_out outputs of `job`
 static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out) {
+  if (job.mode != kProdV) return ws_core(p, job, n_out);
+  return prodv_tail_off(p, job, n_out) + round16(job.plan->runs.size() * 8) + 2 * job.plan->part * prodv_elem_bytes(p);
+}
+static size_t ws_core(const pbc_b200_pairing_s* p, const Job& job, size_t n_out) {
+  // Miller values of a product batch (kProd, kProdV)
+  const size_t n_in = job.mode == kProdV ? job.plan->pairs : n_out * job.k;
+  const bool prod = job.mode == kProd || job.mode == kProdV;
   if (p->type == '1') {
     // f [2], dprod, prefix per output; Miller inputs add f [2], d and the Montgomery P [2]
     const size_t fq = (size_t)kNA1 * 4;
     if (job.mode == kSingle) return n_out * (2 + 1 + 1 + 2) * fq;
-    if (job.mode == kProd) return n_out * job.k * (2 + 1 + 2) * fq + n_out * (2 + 1 + 1) * fq;
+    if (prod) return n_in * (2 + 1 + 2) * fq + n_out * (2 + 1 + 1) * fq;
     return n_out * (2 + 1 + 1) * fq + (p->a1_rows * kNA1 + 4) * 4;
   }
   if (p->type == 'e') {
@@ -233,7 +307,7 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
     // the save [2] and (one-shot) the line table
     const size_t fq = (size_t)kNA1 * 4;
     if (job.mode == kSingle) return n_out * (3 + kQWords + kSWords) * fq;
-    if (job.mode == kProd) return n_out * job.k * (3 + kQWords + kSWords) * fq + n_out * 3 * fq;
+    if (prod) return n_in * (3 + kQWords + kSWords) * fq + n_out * 3 * fq;
     return n_out * (3 + 2) * fq + e_table_bytes(p);
   }
   if (p->type == 'a') {
@@ -243,16 +317,17 @@ static size_t ws_bytes(const pbc_b200_pairing_s* p, const Job& job, size_t n_out
     // products: + vj [3] per pair (V of the pairs that share an accumulator, k_a_miller9_shared)
     if (job.mode == kProd)
       return n_out * job.k * (2 + 1 + 5 + 2 + 3) * fq + n_out * (2 + 1 + 1) * fq;
+    if (job.mode == kProdV) return n_in * (2 + 1 + 5 + 2) * fq + n_out * (2 + 1 + 1) * fq;   // no shared accumulator
     return n_out * (2 + 1 + 1) * fq + (size_t)(3 * (p->a.exp2 + 1) * kNA + 4) * 4;
   }
   // types f, d: Miller values [W][n] words + one flag word each; products add the reduced arrays
   size_t W = p->type == 'f' ? kF12Words : (p->type == 'g' ? kF10Words : 6 * (size_t)p->nlimbs);
-  size_t n_in = job.mode == kProd ? n_out * job.k : n_out;
-  size_t bytes = n_in * (W + 1) * 4;
-  if (p->type == 'f') bytes += n_in * (size_t)kFGWords * 4;   // Q, P of the slot-machine Miller kernel
+  const size_t n_mv = prod ? n_in : n_out;
+  size_t bytes = n_mv * (W + 1) * 4;
+  if (p->type == 'f') bytes += n_mv * (size_t)kFGWords * 4;   // Q, P of the slot-machine Miller kernel
   if (p->type == 'f') bytes += n_out * (size_t)kFStashWords * 4;   // parked F_q^12 values of the slot-machine final exponentiation
   if (job.mode == kPP) bytes += cc_table_bytes(p);             // line table of the fixed first argument
-  if (job.mode == kProd) bytes += n_out * (W + 1) * 4;
+  if (prod) bytes += n_out * (W + 1) * 4;
   return bytes;
 }
 // G1's cofactor (fill_hash) is 1: every point of E(F_q) has order r
@@ -1050,6 +1125,16 @@ static constexpr size_t kSmemEProd = (size_t)kEProdSlots * kSlotA1 * kBlockA1Sma
 static constexpr size_t kSmemEPP = (size_t)kEPPSlots * kSlotA1 * kBlockA1Small;
 static constexpr size_t kSmemEPPInit = (size_t)kEPPInitSlots * kSlotA1 * 32;
 static constexpr size_t kSmemEGroup = (size_t)kEGroupSlots * kSlotA1 * kBlockA1G;
+// the segmented product of pbc_b200_prod_pairings_apply_v (prod_v.cuh): its policies per representation,
+// at the block sizes and slot counts of the uniform product kernels
+using ProdVA = ProdVF2<Ops<kNA, true, kBlockProd>, kNA>;
+using ProdVA1 = ProdVF2<Ops<kNA1, false, kBlockA1Small>, kNA1>;
+using ProdVEl = ProdVE<Ops<kNA1, false, kBlockA1Small>>;
+using ProdVF = ProdVCC<F12ProdV>;
+using ProdVD = ProdVCC<F6DProdV>;
+using ProdVG = ProdVCC<F10ProdV>;
+static_assert((int)ProdVA::kSlots == (int)kAPSlots && (int)ProdVA1::kSlots == kA1ProdSlots && (int)ProdVEl::kSlots == kEProdSlots,
+              "the segmented product runs in the shared memory of the uniform one");
 
 static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
   if ((int)p->ctx.size() <= dev) p->ctx.resize(dev + 1);
@@ -1066,6 +1151,7 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
       CUDA_OK(allow_smem(k_batch_invert<kNA, true, kBlockInv>, kSmemInv16));
       CUDA_OK(allow_smem(k_fpmul_slots<kNA, true, 128, 0>, 2 * 64 * 128));
       CUDA_OK(allow_smem(k_a_prod<kBlockProd>, kSmemAProd));
+      CUDA_OK(allow_smem(k_prod_v<ProdVA, kBlockProd>, kSmemAProd));
       CUDA_OK(allow_smem(k_a_pp_init<32>, kSmemAPPInit));
       CUDA_OK(allow_smem(k_a_pp_apply<kBlockMiller>, kSmemAPPApply));
       CUDA_OK(allow_smem(k_a_g1_mul<kBlockMiller>, (size_t)kGSlots * 64 * kBlockMiller));
@@ -1081,6 +1167,7 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
       CUDA_OK(allow_smem(k_a1_miller<kBlockA1>, kSmemA1Miller));
       CUDA_OK(allow_smem(k_a1_finalexp<kBlockA1Small>, kSmemA1Final));
       CUDA_OK(allow_smem(k_a1_prod<kBlockA1Small>, kSmemA1Prod));
+      CUDA_OK(allow_smem(k_prod_v<ProdVA1, kBlockA1Small>, kSmemA1Prod));
       CUDA_OK(allow_smem(k_a1_pp_init<32>, kSmemA1PPInit));
       CUDA_OK(allow_smem(k_a1_pp_apply<kBlockA1Small>, kSmemA1PP));
       CUDA_OK(allow_smem(k_batch_invert<kNA1, false, kBlockA1Small>, kSmemInv34));
@@ -1095,6 +1182,7 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
     if (p->type == 'e') {
       CUDA_OK(allow_smem(k_e_miller<kBlockE>, kSmemEMiller));
       CUDA_OK(allow_smem(k_e_prod<kBlockA1Small>, kSmemEProd));
+      CUDA_OK(allow_smem(k_prod_v<ProdVEl, kBlockA1Small>, kSmemEProd));
       CUDA_OK(allow_smem(k_e_pp_init<32>, kSmemEPPInit));
       CUDA_OK(allow_smem(k_e_pp_apply<kBlockA1Small>, kSmemEPP));
       CUDA_OK(allow_smem(k_e_finalexp<kBlockA1Small>, kSmemEFinal));
@@ -1169,6 +1257,10 @@ static void ctx_release(DevCtx& c) {
   }
   cudaFree(c.ws_dev);
   if (c.ws_ev) cudaEventDestroy(c.ws_ev);
+  for (int s = 0; s < DevCtx::kPlanSlots; s++) {
+    if (c.plan_ev[s]) { cudaEventSynchronize(c.plan_ev[s]); cudaEventDestroy(c.plan_ev[s]); }
+    cudaFreeHost(c.plan_h[s]);
+  }
   for (int i = 0; i < 4; i++) if (c.ev[i]) cudaEventDestroy(c.ev[i]);
   c = DevCtx();
 }
@@ -1183,6 +1275,29 @@ static int ws_release(DevCtx& c, cudaStream_t st) {
   CUDA_OK(cudaEventRecord(c.ws_ev, st));
   c.ws_used = true;
   return 0;
+}
+
+// kProdV: copy the run tables of `job` to `dst` (device memory) on `st` through the next pinned slot
+static int upload_plan(DevCtx& c, const Job& job, void* dst, cudaStream_t st) {
+  const int s = c.plan_next;
+  c.plan_next = (s + 1) % DevCtx::kPlanSlots;
+  if (!c.plan_ev[s]) CUDA_OK(cudaEventCreateWithFlags(&c.plan_ev[s], cudaEventDisableTiming));
+  else CUDA_OK(cudaEventSynchronize(c.plan_ev[s]));     // the slot's last upload has run
+  const size_t bytes = job.plan->runs.size() * 8;
+  if (c.plan_cap[s] < bytes) {
+    cudaFreeHost(c.plan_h[s]);
+    c.plan_h[s] = nullptr;
+    c.plan_cap[s] = 0;
+    CUDA_OK(cudaHostAlloc(&c.plan_h[s], bytes, cudaHostAllocPortable));
+    c.plan_cap[s] = bytes;
+  }
+  memcpy(c.plan_h[s], job.plan->runs.data(), bytes);
+  CUDA_OK(cudaMemcpyAsync(dst, c.plan_h[s], bytes, cudaMemcpyHostToDevice, st));
+  CUDA_OK(cudaEventRecord(c.plan_ev[s], st));
+  return 0;
+}
+static uint64_t* prodv_runs(const pbc_b200_pairing_s* p, const Job& job, void* ws, size_t n_out) {
+  return (uint64_t*)((uint8_t*)ws + prodv_tail_off(p, job, n_out));
 }
 
 // multiprocessors of the current device, as ctx_prepare read them
@@ -1230,6 +1345,51 @@ static int enqueue_final(pbc_b200_pairing_s* p, void* f, void* dprod, void* pref
 }
 
 // ------------------------------------------------------------------------------------------
+// kProdV: the passes of the segmented product (prod_v.cuh) from the Miller values `mil` to the layout
+// the final stage reads (`fin`, one element per output).  The run tables are in the workspace
+// (upload_plan), the two partial-product buffers after them.
+// ------------------------------------------------------------------------------------------
+static int enqueue_prod_v(pbc_b200_pairing_s* p, const Job& job, ProdVBuf mil, ProdVBuf fin, void* ws, size_t n,
+                          cudaStream_t st) {
+  const ProdPlan& pl = *job.plan;
+  const uint64_t* runs = prodv_runs(p, job, ws, n);
+  const size_t eb = prodv_elem_bytes(p), cap = pl.part;
+  // value rows first, validity after them (the Miller kernels' order)
+  const size_t vb = prodv_value_bytes(p);
+  uint8_t* base = (uint8_t*)runs + round16(pl.runs.size() * 8);
+  ProdVBuf part[2];
+  for (int b = 0; b < 2; b++) {
+    uint8_t* v = base + b * cap * eb;
+    part[b] = ProdVBuf{v, v + vb * cap, cap};
+  }
+  ProdVBuf in = mil;
+  size_t off = 0;
+  for (size_t s = 0; s < pl.count.size(); off += pl.count[s] + 1, s++) {
+    const int last = s + 1 == pl.count.size();
+    const ProdVBuf out = last ? fin : part[s & 1];
+    const size_t R = pl.count[s];
+    const uint64_t* r = runs + off;
+    if (p->type == 'a')
+      k_prod_v<ProdVA, kBlockProd><<<(unsigned)((R + kBlockProd - 1) / kBlockProd), kBlockProd, kSmemAProd, st>>>(in, out, r, R, last);
+    else if (p->type == '1')
+      k_prod_v<ProdVA1, kBlockA1Small><<<(unsigned)((R + kBlockA1Small - 1) / kBlockA1Small), kBlockA1Small, kSmemA1Prod, st>>>(in, out, r, R, last);
+    else if (p->type == 'e')
+      k_prod_v<ProdVEl, kBlockA1Small><<<(unsigned)((R + kBlockA1Small - 1) / kBlockA1Small), kBlockA1Small, kSmemEProd, st>>>(in, out, r, R, last);
+    else if (p->dwide)
+      pbcb200_dw::dw_prod_v((const uint32_t*)in.v, (const uint32_t*)in.d, in.n, (uint32_t*)out.v, (uint32_t*)out.d, out.n, r, R, st);
+    else if (p->type == 'f')
+      k_prod_v<ProdVF, kBlockCC><<<(unsigned)((R + kBlockCC - 1) / kBlockCC), kBlockCC, 0, st>>>(in, out, r, R, last);
+    else if (p->type == 'g')
+      k_prod_v<ProdVG, kBlockCC><<<(unsigned)((R + kBlockCC - 1) / kBlockCC), kBlockCC, 0, st>>>(in, out, r, R, last);
+    else
+      k_prod_v<ProdVD, kBlockCC><<<(unsigned)((R + kBlockCC - 1) / kBlockCC), kBlockCC, 0, st>>>(in, out, r, R, last);
+    LAUNCHED();
+    in = out;
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
 // enqueue one batch of n_out outputs of `job`, device buffers, on `st`.  ws: ws_bytes() bytes.
 // ------------------------------------------------------------------------------------------
 static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_out, const uint8_t* d_in1,
@@ -1251,8 +1411,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       unsigned gm = (unsigned)((n + kBlockA1 - 1) / kBlockA1);
       k_a1_miller<kBlockA1><<<gm, kBlockA1, kSmemA1Miller, st>>>(d_in1, d_in2, f, dprod, pm, n, wire);
       LAUNCHED();
-    } else if (job.mode == kProd) {
-      size_t m = n * job.k;
+    } else if (job.mode == kProd || job.mode == kProdV) {
+      size_t m = job.mode == kProd ? n * job.k : job.plan->pairs;
       uint2* fi = (uint2*)ws;                    // [2][E][m]
       uint2* di = fi + 2 * E * m;                // [E][m]
       uint2* pm = di + E * m;                    // [2][E][m]
@@ -1262,9 +1422,13 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       unsigned gm = (unsigned)((m + kBlockA1 - 1) / kBlockA1);
       k_a1_miller<kBlockA1><<<gm, kBlockA1, kSmemA1Miller, st>>>(d_in1, d_in2, fi, di, pm, m, wire);
       LAUNCHED();
-      unsigned gp = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
-      k_a1_prod<kBlockA1Small><<<gp, kBlockA1Small, kSmemA1Prod, st>>>(fi, di, f, dprod, job.k, n, m);
-      LAUNCHED();
+      if (job.mode == kProdV) {
+        if (enqueue_prod_v(p, job, ProdVBuf{fi, di, m}, ProdVBuf{f, dprod, n}, ws, n, st)) return 1;
+      } else {
+        unsigned gp = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
+        k_a1_prod<kBlockA1Small><<<gp, kBlockA1Small, kSmemA1Prod, st>>>(fi, di, f, dprod, job.k, n, m);
+        LAUNCHED();
+      }
     } else {
       f = (uint2*)ws;
       dprod = f + 2 * E * n;
@@ -1288,8 +1452,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     uint2 *f, *dprod, *prefix;
     const size_t wire = (size_t)p->g1_len;
     STAGE(0);
-    if (job.mode == kSingle || job.mode == kProd) {
-      const size_t m = job.mode == kProd ? n * job.k : n;
+    if (job.mode != kPP) {
+      const size_t m = job.mode == kProd ? n * job.k : (job.mode == kProdV ? job.plan->pairs : n);
       uint2* fi = (uint2*)ws;                    // [E][m]
       uint2* di = fi + E * m;                    // [E][m]
       uint2* px = di + E * m;                    // [E][m]
@@ -1306,9 +1470,13 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
         f = sv + kSWords * E * m;                // [E][n]
         dprod = f + E * n;
         prefix = dprod + E * n;
-        unsigned gp = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
-        k_e_prod<kBlockA1Small><<<gp, kBlockA1Small, kSmemEProd, st>>>(fi, di, f, dprod, job.k, n, m);
-        LAUNCHED();
+        if (job.mode == kProdV) {
+          if (enqueue_prod_v(p, job, ProdVBuf{fi, di, m}, ProdVBuf{f, dprod, n}, ws, n, st)) return 1;
+        } else {
+          unsigned gp = (unsigned)((n + kBlockA1Small - 1) / kBlockA1Small);
+          k_e_prod<kBlockA1Small><<<gp, kBlockA1Small, kSmemEProd, st>>>(fi, di, f, dprod, job.k, n, m);
+          LAUNCHED();
+        }
       }
     } else {
       f = (uint2*)ws;
@@ -1371,6 +1539,20 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       unsigned gp = (unsigned)((n + kBlockProd - 1) / kBlockProd);
       k_a_prod<kBlockProd><<<gp, kBlockProd, kSmemAProd, st>>>(fi, di, f, dprod, kk, n, mm);
       LAUNCHED();
+    } else if (job.mode == kProdV) {
+      // one k_a_miller9 thread per pair (no shared accumulator), then the segmented product
+      const size_t m = job.plan->pairs;
+      uint4* fi = (uint4*)ws;                    // [2][4][m]
+      uint4* di = fi + 8 * m;                    // [4][m]
+      uint4* save = di + 4 * m;                  // [5][4][m]
+      uint4* qm = save + 20 * m;                 // [2][4][m]
+      f = qm + 8 * m;                            // [2][4][n]
+      dprod = f + 8 * n;
+      prefix = dprod + 4 * n;
+      unsigned gm = (unsigned)((m + kBlockMiller - 1) / kBlockMiller);
+      k_a_miller9<kBlockMiller><<<gm, kBlockMiller, kSmemAMiller9, st>>>(d_in1, d_in2, fi, di, save, qm, m);
+      LAUNCHED();
+      if (enqueue_prod_v(p, job, ProdVBuf{fi, di, m}, ProdVBuf{f, dprod, n}, ws, n, st)) return 1;
     } else {
       f = (uint4*)ws;
       dprod = f + 8 * n;
@@ -1391,7 +1573,8 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
   if (p->type == 'f' || p->type == 'd' || p->type == 'g') {
     const bool isf = p->type == 'f', isg = p->type == 'g', wide = p->dwide;
     const size_t W = isf ? kF12Words : (isg ? kF10Words : 6 * (size_t)p->nlimbs);
-    size_t m = job.mode == kProd ? n * job.k : n;
+    const bool prod = job.mode == kProd || job.mode == kProdV;
+    size_t m = job.mode == kProd ? n * job.k : (job.mode == kProdV ? job.plan->pairs : n);
     uint32_t* mv = (uint32_t*)ws;                // [W][m]
     uint32_t* flag = mv + W * m;                 // [m]
     size_t stride1 = job.mode == kPP ? 0 : (size_t)p->g1_len;
@@ -1415,7 +1598,7 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
     }
     if (wide) pbcb200_dw::dw_miller(d_in1, d_in2, mv, flag, m, stride1, tab, rows, st);
     else if (isf && p->f.slots_ok) {
-      uint32_t* gq = mv + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0);   // after the Miller values and flags
+      uint32_t* gq = mv + (W + 1) * m + (prod ? (W + 1) * n : 0);   // after the Miller values and flags
       k_f_miller_s<kBlockFSM><<<(unsigned)((m + kBlockFSM - 1) / kBlockFSM), kBlockFSM, kSmemFMillerS, st>>>(d_in1, d_in2, mv, flag, gq, m, stride1, tab, rows);
     } else if (isf) k_f_miller<kBlockCCMiller><<<gm, kBlockCCMiller, 0, st>>>(d_in1, d_in2, mv, flag, m, stride1, tab, rows);
     else if (isg) k_g_miller<kBlockCCMiller><<<gm, kBlockCCMiller, 0, st>>>(d_in1, d_in2, mv, flag, m, stride1, tab, rows);
@@ -1432,13 +1615,18 @@ static int enqueue_pairings(pbc_b200_pairing_s* p, const Job& job, uint8_t* d_ou
       else k_d_prod<kBlockCC><<<gp, kBlockCC, 0, st>>>(mv, flag, mvo, flago, job.k, n, m);
       LAUNCHED();
       mv = mvo; flag = flago;
+    } else if (job.mode == kProdV) {
+      uint32_t* mvo = flag + m;                  // [W][n]
+      uint32_t* flago = mvo + W * n;
+      if (enqueue_prod_v(p, job, ProdVBuf{mv, flag, m}, ProdVBuf{mvo, flago, n}, ws, n, st)) return 1;
+      mv = mvo; flag = flago;
     }
     STAGE(2);
     unsigned gf = (unsigned)((n + kBlockCC - 1) / kBlockCC);
     unsigned gfm = (unsigned)((n + kBlockCCMiller - 1) / kBlockCCMiller);
     if (wide) pbcb200_dw::dw_finalexp(mv, flag, d_out, n, st);
     else if (isf && p->f.slots_ok && p->f.bn) {
-      uint32_t* stash = (uint32_t*)ws + (W + 1) * m + (job.mode == kProd ? (W + 1) * n : 0) + (size_t)kFGWords * m;
+      uint32_t* stash = (uint32_t*)ws + (W + 1) * m + (prod ? (W + 1) * n : 0) + (size_t)kFGWords * m;
       k_f_finalexp_s<kBlockFS><<<(unsigned)((n + kBlockFS - 1) / kBlockFS), kBlockFS, kSmemFFinalS, st>>>(mv, flag, d_out, stash, n);
     } else if (isf) k_f_finalexp<kBlockCCMiller><<<gfm, kBlockCCMiller, 0, st>>>(mv, flag, d_out, n);
     else if (isg) k_g_finalexp<kBlockCCMiller><<<gfm, kBlockCCMiller, 0, st>>>(mv, flag, d_out, n);
@@ -1524,6 +1712,103 @@ static int run_host(pbc_b200_pairing_s* p, const Job& job, unsigned char* out, c
   return 0;
 }
 
+// (re)allocate a device buffer to at least `need` bytes
+static int grow(void** buf, size_t* cap, size_t need) {
+  if (*cap >= need) return 0;
+  cudaFree(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  CUDA_OK(cudaMalloc(buf, need));
+  *cap = need;
+  return 0;
+}
+
+// host-buffer pipeline of pbc_b200_prod_pairings_apply_v on one device: outputs [0, n) with pairs
+// [off[0], off[n]) (in1, in2 point at pair off[0]).  Chunks hold whole outputs, packed while their pair
+// count stays at or below kChunk; an output with more pairs is a chunk of its own.  Two streams, as
+// run_slice.
+static int run_slice_v(pbc_b200_pairing_s* p, int dev, unsigned char* out, const unsigned char* in1,
+                       const unsigned char* in2, const size_t* off, size_t n) {
+  std::lock_guard<std::mutex> dev_lock(g_dev_mu[dev & 63]);
+  if (ctx_prepare(p, dev)) return 1;
+  DevCtx& c = p->ctx[dev];
+  std::vector<size_t> lo{0};                     // first output of every chunk, then n
+  for (size_t i = 0; i < n;) {
+    size_t j = i + 1;
+    while (j < n && off[j + 1] - off[i] <= kChunk) j++;
+    lo.push_back(j);
+    i = j;
+  }
+  const size_t chunks = lo.size() - 1;
+  std::vector<ProdPlan> plan(chunks);
+  size_t b1 = 0, b2 = 0, bo = 0, bw = 0;
+  for (size_t k = 0; k < chunks; k++) {
+    plan[k] = prod_plan(off + lo[k], lo[k + 1] - lo[k]);
+    Job job{kProdV, 1, &plan[k]};
+    b1 = std::max(b1, plan[k].pairs * p->g1_len);
+    b2 = std::max(b2, plan[k].pairs * p->g2_len);
+    bo = std::max(bo, (lo[k + 1] - lo[k]) * p->gt_len);
+    bw = std::max(bw, ws_bytes(p, job, lo[k + 1] - lo[k]));
+  }
+  for (int s = 0; s < 2 && s < (int)chunks; s++) {
+    if (grow((void**)&c.d_in1[s], &c.cap_in1[s], b1) || grow((void**)&c.d_in2[s], &c.cap_in2[s], b2) ||
+        grow((void**)&c.d_out[s], &c.cap_out[s], bo) || grow(&c.ws[s], &c.cap_ws[s], bw)) return 1;
+  }
+  for (size_t k = 0; k < chunks; k++) {
+    const int s = k & 1;
+    cudaStream_t st = c.stream[s];
+    const size_t m = lo[k + 1] - lo[k], j0 = off[lo[k]] - off[0];
+    const Job job{kProdV, 1, &plan[k]};
+    CUDA_OK(cudaMemcpyAsync(c.d_in1[s], in1 + j0 * p->g1_len, plan[k].pairs * p->g1_len, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(c.d_in2[s], in2 + j0 * p->g2_len, plan[k].pairs * p->g2_len, cudaMemcpyHostToDevice, st));
+    if (upload_plan(c, job, prodv_runs(p, job, c.ws[s], m), st)) return 1;
+    if (enqueue_pairings(p, job, c.d_out[s], c.d_in1[s], c.d_in2[s], m, c.ws[s], st)) return 1;
+    CUDA_OK(cudaMemcpyAsync(out + lo[k] * p->gt_len, c.d_out[s], m * p->gt_len, cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_OK(cudaStreamSynchronize(c.stream[0]));
+  CUDA_OK(cudaStreamSynchronize(c.stream[1]));
+  return 0;
+}
+
+// first output of device g's slice: the first i with off[i] world >= g off[n] (pairs, not outputs, are
+// balanced); g = world gives n
+static size_t slice_start_v(const size_t* off, size_t n, int g, int world) {
+  const unsigned __int128 goal = (unsigned __int128)g * off[n];
+  size_t a = 0, b = n;                           // off is increasing: binary search
+  while (a < b) {
+    const size_t mid = a + (b - a) / 2;
+    if ((unsigned __int128)off[mid] * (unsigned)world >= goal) b = mid; else a = mid + 1;
+  }
+  return a;
+}
+
+// contiguous slices of the outputs, balanced by pairs, one host thread per device (as run_host)
+static int run_host_v(pbc_b200_pairing_s* p, unsigned char* out, const unsigned char* in1, const unsigned char* in2,
+                      const size_t* off, size_t n) {
+  if (!out || !in1 || !in2) return fail("null argument");
+  std::lock_guard<std::mutex> lk(p->mu);
+  int cur = 0;
+  CUDA_OK(cudaGetDevice(&cur));
+  if (p->ndev <= 1) return run_slice_v(p, cur, out, in1, in2, off, n);
+  const int nd = p->ndev;
+  if ((int)p->ctx.size() < nd) p->ctx.resize(nd);
+  std::vector<int> rc(nd, 0);
+  std::vector<std::string> msg(nd);
+  std::vector<std::thread> th;
+  for (int d = 0; d < nd; d++) {
+    const size_t lo = slice_start_v(off, n, d, nd), hi = slice_start_v(off, n, d + 1, nd);
+    if (lo >= hi) continue;
+    th.emplace_back([=, &rc, &msg]() {
+      rc[d] = run_slice_v(p, d, out + lo * p->gt_len, in1 + off[lo] * p->g1_len, in2 + off[lo] * p->g2_len, off + lo, hi - lo);
+      if (rc[d]) msg[d] = g_err;
+    });
+  }
+  for (auto& t : th) t.join();
+  cudaSetDevice(cur);
+  for (int d = 0; d < nd; d++) if (rc[d]) return fail("device %d: %s", d, msg[d].c_str());
+  return 0;
+}
+
 static int run_device(pbc_b200_pairing_s* p, const Job& job, void* d_out, const void* d_in1,
                       const void* d_in2, size_t n, void* stream) {
   if (!p) return fail("null argument");
@@ -1544,6 +1829,7 @@ static int run_device(pbc_b200_pairing_s* p, const Job& job, void* d_out, const 
   if (p->profile && !c.ev[0])
     for (int i = 0; i < 4; i++) CUDA_OK(cudaEventCreate(&c.ev[i]));
   if (ws_acquire(c, (cudaStream_t)stream)) return 1;
+  if (job.mode == kProdV && upload_plan(c, job, prodv_runs(p, job, c.ws_dev, n), (cudaStream_t)stream)) return 1;
   if (enqueue_pairings(p, job, (uint8_t*)d_out, (const uint8_t*)d_in1, (const uint8_t*)d_in2, n,
                        c.ws_dev, (cudaStream_t)stream, p->profile ? c.ev : nullptr)) return 1;
   return ws_release(c, (cudaStream_t)stream);
@@ -1654,6 +1940,37 @@ int pbc_b200_prod_pairings_apply_device(pbc_b200_pairing_t* p, void* d_out, cons
                                         const void* d_in2, size_t k, size_t n_out, void* stream) {
   if (k == 0) return fail("prod_pairings: k must be positive");
   return run_device(p, Job{kProd, k}, d_out, d_in1, d_in2, n_out, stream);
+}
+
+// offsets of pbc_b200_prod_pairings_apply_v: checked before any CUDA call
+static int check_offsets(const pbc_b200_pairing_s* p, const size_t* off, size_t n_out) {
+  if (!off) return fail("prod_pairings_v: offsets is NULL");
+  if (off[0] != 0) return fail("prod_pairings_v: offsets[0] must be 0 (got %zu)", off[0]);
+  for (size_t i = 1; i <= n_out; i++)
+    if (off[i] <= off[i - 1])
+      return fail("prod_pairings_v: offsets[%zu] = %zu is not above offsets[%zu] = %zu (every output needs at least one pair)",
+                  i, off[i], i - 1, off[i - 1]);
+  const size_t wide = (size_t)(p->g1_len > p->g2_len ? p->g1_len : p->g2_len);
+  if (off[n_out] > SIZE_MAX / wide || n_out > SIZE_MAX / (size_t)p->gt_len)
+    return fail("prod_pairings_v: %zu pairs / %zu outputs overflow the byte count", off[n_out], n_out);
+  return 0;
+}
+
+int pbc_b200_prod_pairings_apply_v(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in1,
+                                   const unsigned char* in2, const size_t* offsets, size_t n_out) {
+  if (!p) return fail("null argument");
+  if (n_out == 0) return 0;
+  if (check_offsets(p, offsets, n_out)) return 1;
+  return run_host_v(p, out, in1, in2, offsets, n_out);
+}
+
+int pbc_b200_prod_pairings_apply_v_device(pbc_b200_pairing_t* p, void* d_out, const void* d_in1, const void* d_in2,
+                                          const size_t* offsets, size_t n_out, void* stream) {
+  if (!p) return fail("null argument");
+  if (n_out == 0) return 0;
+  if (check_offsets(p, offsets, n_out)) return 1;
+  const ProdPlan plan = prod_plan(offsets, n_out);
+  return run_device(p, Job{kProdV, 1, &plan}, d_out, d_in1, d_in2, n_out, stream);
 }
 
 int pbc_b200_pp_pairings_apply(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in1,

@@ -54,6 +54,11 @@ void dw_prod(const uint32_t* mv, const uint32_t* flag, uint32_t* mvo, uint32_t* 
              size_t m, cudaStream_t st) {
   k_d_prod<kBlockW><<<grid(n, kBlockW), kBlockW, 0, st>>>(mv, flag, mvo, flago, k, n, m);
 }
+void dw_prod_v(const uint32_t* mv, const uint32_t* flag, size_t n, uint32_t* mvo, uint32_t* flago, size_t n_o,
+               const uint64_t* runs, size_t n_runs, cudaStream_t st) {
+  k_prod_v<ProdVCC<F6DProdV>, kBlockW><<<grid(n_runs, kBlockW), kBlockW, 0, st>>>(
+      ProdVBuf{(void*)mv, (void*)flag, n}, ProdVBuf{mvo, flago, n_o}, runs, n_runs, 1);
+}
 void dw_finalexp(const uint32_t* mv, const uint32_t* flag, uint8_t* out, size_t n, cudaStream_t st) {
   k_d_finalexp<kBlockW><<<grid(n, kBlockW), kBlockW, 0, st>>>(mv, flag, out, n);
 }

@@ -24,6 +24,10 @@ void dw_miller(const uint8_t* P, const uint8_t* Q, uint32_t* mv, uint32_t* flag,
                const uint32_t* tab, size_t rows, cudaStream_t st);
 void dw_prod(const uint32_t* mv, const uint32_t* flag, uint32_t* mvo, uint32_t* flago, size_t k, size_t n,
              size_t m, cudaStream_t st);
+// one pass of the segmented product (prod_v.cuh): runs[r] .. runs[r + 1] of (mv, flag), stride n, into
+// element r of (mvo, flago), stride n_o
+void dw_prod_v(const uint32_t* mv, const uint32_t* flag, size_t n, uint32_t* mvo, uint32_t* flago, size_t n_o,
+               const uint64_t* runs, size_t n_runs, cudaStream_t st);
 void dw_finalexp(const uint32_t* mv, const uint32_t* flag, uint8_t* out, size_t n, cudaStream_t st);
 void dw_pp_init(const uint8_t* P, uint32_t* tab, size_t rows, cudaStream_t st);
 // which: 0 = G1, 1 = GT, 2 = G2 (as engine.cu's enqueue_group)

@@ -16,6 +16,7 @@
 #pragma once
 #include "slots.cuh"
 #include "a_steps.cuh"
+#include "prod_v.cuh"
 
 namespace pbcb200 {
 

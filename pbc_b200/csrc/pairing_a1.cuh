@@ -21,6 +21,7 @@
 #pragma once
 #include "common_kernels.cuh"
 #include "a_steps.cuh"
+#include "prod_v.cuh"
 
 namespace pbcb200 {
 

@@ -10,6 +10,7 @@
 // constants x^q, x^(2q) the reference already computes (ecc/d_param.c:1043-1049).
 #pragma once
 #include "miller_cc.cuh"
+#include "prod_v.cuh"
 
 namespace pbcb200 {
 
@@ -415,6 +416,16 @@ k_d_prod(const uint32_t* __restrict__ mv_in, const uint32_t* __restrict__ flag_i
   f6d_st_global(mv_out, n_out, idx, acc);
   flag_out[idx] = ok ? 1u : 0u;
 }
+
+// the same product over a run table (prod_v.cuh, pbc_b200_prod_pairings_apply_v)
+struct F6DProdV {
+  using E = F6D;
+  // eight limbs (engine_d_wide.cu): at kCCMinBlocks the 128-register cap spills the accumulator
+  static constexpr int kMinBlocks = kNS > 5 ? 3 : kCCMinBlocks;
+  static __device__ __forceinline__ void ld(E& v, const uint32_t* g, size_t n, size_t i) { f6d_ld_global(v, g, n, i); }
+  static __device__ __forceinline__ void st(uint32_t* g, size_t n, size_t i, const E& v) { f6d_st_global(g, n, i, v); }
+  static __device__ __forceinline__ void mul(E* r, const E* x, const E* y) { f6d_mul(r, x, y); }
+};
 
 // cc_tatepower, k = 6 branch (ecc/d_param.c:505-564) followed by lucas_even (:441-502)
 __device__ __noinline__ void f6d_final_exp(F3& out0, F3& out1, F6D& f) {

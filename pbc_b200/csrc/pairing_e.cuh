@@ -31,6 +31,7 @@
 // The 34-limb slot machine, wire conversion, scalar decoding and table rows are type A1's.
 #pragma once
 #include "pairing_a1.cuh"
+#include "prod_v.cuh"
 
 namespace pbcb200 {
 
@@ -333,6 +334,29 @@ k_e_prod(const void* __restrict__ f_in, const void* __restrict__ d_in, void* __r
   e_publish<O>(pF, pD, valid, f_out, d_out, n_out, idx);
 }
 constexpr int kEProdSlots = 3;
+
+// the same product over a run table (prod_v.cuh, pbc_b200_prod_pairings_apply_v): numerator and
+// denominator multiplied separately; every pass stores through e_publish (vd = 0 marks an invalid pair)
+template <class O>
+struct ProdVE {
+  enum { pF, pD, pT, kSlots };
+  static constexpr int kMinBlocks = 1;
+  bool ok;
+  __device__ __forceinline__ void first(const ProdVBuf& in, size_t j) {
+    O::ld_global(pF, in.v, 0, in.n, j);
+    O::ld_global(pD, in.d, 0, in.n, j);
+    ok = !O::is_zero(pD);
+  }
+  __device__ __forceinline__ void next(const ProdVBuf& in, size_t j) {
+    O::ld_global(pT, in.d, 0, in.n, j);
+    ok = ok && !O::is_zero(pT);
+    O::mul(pD, pD, pT);
+    O::mulg(pF, pF, e_el(in.v, 0, in.n, j), in.n);
+  }
+  __device__ __forceinline__ void store(const ProdVBuf& out, size_t r, bool) {
+    e_publish<O>(pF, pD, ok, out.v, out.d, out.n, r);
+  }
+};
 
 // ---- fixed first argument ----
 // Table rows (34 words each, Montgomery form), for step i < exp2: 5 i + {a, b, c} of the tangent,

@@ -17,6 +17,7 @@
 // of k Miller values), k_f_finalexp.
 #pragma once
 #include "miller_cc.cuh"
+#include "prod_v.cuh"
 
 namespace pbcb200 {
 
@@ -509,6 +510,15 @@ k_f_prod(const uint32_t* __restrict__ mv_in, const uint32_t* __restrict__ flag_i
   f12_st_global(mv_out, n_out, idx, acc);
   flag_out[idx] = ok ? 1u : 0u;
 }
+
+// the same product over a run table (prod_v.cuh, pbc_b200_prod_pairings_apply_v)
+struct F12ProdV {
+  using E = F12;
+  static constexpr int kMinBlocks = kCCMinBlocks;
+  static __device__ __forceinline__ void ld(E& v, const uint32_t* g, size_t n, size_t i) { f12_ld_global(v, g, n, i); }
+  static __device__ __forceinline__ void st(uint32_t* g, size_t n, size_t i, const E& v) { f12_st_global(g, n, i, v); }
+  static __device__ __forceinline__ void mul(E* r, const E* x, const E* y) { f12_mul(r, x, y); }
+};
 
 // f^(q^6): x -> -x
 __device__ __forceinline__ void f12_conj(F12& r, const F12& f) {

@@ -13,6 +13,7 @@
 // Wire format: 19 bytes per F_q coordinate (not a multiple of four: byte-wise conversion).
 #pragma once
 #include "miller_cc.cuh"
+#include "prod_v.cuh"
 
 namespace pbcb200 {
 
@@ -302,6 +303,15 @@ k_g_prod(const uint32_t* __restrict__ mv_in, const uint32_t* __restrict__ flag_i
   f10_st_global(mv_out, n_out, idx, acc);
   flag_out[idx] = ok ? 1u : 0u;
 }
+
+// the same product over a run table (prod_v.cuh, pbc_b200_prod_pairings_apply_v)
+struct F10ProdV {
+  using E = F10;
+  static constexpr int kMinBlocks = kCCMinBlocks;
+  static __device__ __forceinline__ void ld(E& v, const uint32_t* g, size_t n, size_t i) { f10_ld_global(v, g, n, i); }
+  static __device__ __forceinline__ void st(uint32_t* g, size_t n, size_t i, const E& v) { f10_st_global(g, n, i, v); }
+  static __device__ __forceinline__ void mul(E* r, const E* x, const E* y) { f10_mul(r, x, y); }
+};
 
 // tatepower10 (ecc/g_param.c:471-536) followed by lucas_even (:413-469)
 __device__ __noinline__ void f10_final_exp(F5& out0, F5& out1, F10& f) {

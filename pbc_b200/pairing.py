@@ -2,7 +2,8 @@
 
 Names follow the reference (include/pbc_pairing.h): a `Pairing` is a pairing_t initialised from
 parameter text (pairing_init_set_str); `apply` is element_pairing over a batch;
-`prod_apply` is element_prod_pairing; `pp_apply` is pairing_pp_init + pairing_pp_apply.
+`prod_apply` is element_prod_pairing (k pairs per output), `prod_apply_v` the same with a pair count
+per output (ragged batches); `pp_apply` is pairing_pp_init + pairing_pp_apply.
 Elements travel as reference wire-format bytes (element_to_bytes / element_from_bytes).
 All arithmetic happens in libpbc_b200.so on the GPU; this file only marshals buffers.
 """
@@ -114,6 +115,44 @@ class Pairing:
 
     def prod_apply_device(self, d_out, d_in1, d_in2, k, n_out, stream=0):
         if lib.pbc_b200_prod_pairings_apply_device(self._h, d_out, d_in1, d_in2, k, n_out, stream):
+            raise PairingError(last_error())
+
+    # -- element_prod_pairing with a pair count per output ---------------------------------------
+    @staticmethod
+    def _offsets(offsets):
+        """offsets (any integer sequence or numpy array, n_out + 1 entries) as a C size_t array; the
+        library checks that they start at 0 and increase"""
+        vals = offsets.tolist() if hasattr(offsets, "tolist") else list(offsets)
+        if not vals:
+            raise ValueError("offsets: n_out + 1 entries needed")
+        if any(isinstance(v, bool) or not isinstance(v, int) or v < 0 for v in vals):
+            raise ValueError("offsets: non-negative integers needed")
+        return (C.c_size_t * len(vals))(*vals), len(vals) - 1
+
+    def prod_apply_v(self, in1: bytes, in2: bytes, offsets) -> bytes:
+        """out[i] = prod of e(in1[j], in2[j]) over offsets[i] <= j < offsets[i+1]"""
+        offs, n_out = self._offsets(offsets)
+        m = offs[n_out]
+        self._need(in1, m * self.g1_len, "prod_apply_v in1")
+        self._need(in2, m * self.g2_len, "prod_apply_v in2")
+        out = C.create_string_buffer(max(1, n_out * self.gt_len))
+        if lib.pbc_b200_prod_pairings_apply_v(self._h, C.addressof(out), _addr(in1), _addr(in2), C.addressof(offs), n_out):
+            raise PairingError(last_error())
+        return out.raw[:n_out * self.gt_len]
+
+    def prod_apply_v_into(self, out, in1, in2, offsets):
+        offs, n_out = self._offsets(offsets)
+        m = offs[n_out]
+        self._need(out, n_out * self.gt_len, "prod_apply_v out")
+        self._need(in1, m * self.g1_len, "prod_apply_v in1")
+        self._need(in2, m * self.g2_len, "prod_apply_v in2")
+        if lib.pbc_b200_prod_pairings_apply_v(self._h, _addr(out), _addr(in1), _addr(in2), C.addressof(offs), n_out):
+            raise PairingError(last_error())
+
+    def prod_apply_v_device(self, d_out, d_in1, d_in2, offsets, stream=0):
+        """device pointers, offsets on the host; asynchronous on `stream`"""
+        offs, n_out = self._offsets(offsets)
+        if lib.pbc_b200_prod_pairings_apply_v_device(self._h, d_out, d_in1, d_in2, C.addressof(offs), n_out, stream):
             raise PairingError(last_error())
 
     # -- pairing_pp_init / pairing_pp_apply -------------------------------------------------------

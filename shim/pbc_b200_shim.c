@@ -16,6 +16,7 @@
  *       the reference's.  A caller such as benchmark/benchmark.c compiles and links unchanged.
  *   pbc_b200_pairing_batch / pbc_b200_prod_pairing_batch -- the additive batch entry points
  *       (SURVEY 8b): n pairings in one call, reference wire format in and out.
+ *   pbc_b200_prod_pairing_batch_v -- products with a pair count per output (offsets, host memory).
  *   element_pairing_batch -- the same over arrays of element_t.
  *
  * Elements cross the boundary as the bytes element_to_bytes() writes (include/pbc_field.h:475-484),
@@ -187,6 +188,12 @@ int pbc_b200_pairing_batch(pairing_t pairing, unsigned char *out, const unsigned
 int pbc_b200_prod_pairing_batch(pairing_t pairing, unsigned char *out, const unsigned char *in1,
                                 const unsigned char *in2, int n_prod, size_t n_out) {
   return pbc_b200_prod_pairings_apply(find_attach(pairing)->h, out, in1, in2, (size_t)n_prod, n_out);
+}
+/* out[i] = prod_{offsets[i] <= j < offsets[i+1]} e(in1[j], in2[j]): one GPU call for products of
+ * different lengths (include/pbc_b200.h, pbc_b200_prod_pairings_apply_v) */
+int pbc_b200_prod_pairing_batch_v(pairing_t pairing, unsigned char *out, const unsigned char *in1,
+                                  const unsigned char *in2, const size_t *offsets, size_t n_out) {
+  return pbc_b200_prod_pairings_apply_v(find_attach(pairing)->h, out, in1, in2, offsets, n_out);
 }
 
 /* out[i] = e(in1[i], in2[i]) for arrays of element_t: one GPU batch instead of n element_pairing

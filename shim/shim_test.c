@@ -17,6 +17,8 @@ void element_pairing_batch(element_t out[], element_t in1[], element_t in2[], in
 void element_pow_zn_batch(element_t out[], element_t in[], element_t k[], int n);
 int pbc_b200_pairing_batch(pairing_t pairing, unsigned char *out, const unsigned char *in1,
                            const unsigned char *in2, size_t n);
+int pbc_b200_prod_pairing_batch_v(pairing_t pairing, unsigned char *out, const unsigned char *in1,
+                                  const unsigned char *in2, const size_t *offsets, size_t n_out);
 
 static int same(element_t a, element_t b) {
   unsigned char x[1024], y[1024];
@@ -72,6 +74,27 @@ int main(int argc, char **argv) {
     if (!same(ep, e2)) { printf("element_prod_pairing mismatch\n"); bad++; }
     for (i = 0; i < 4; i++) { element_clear(pc[i]); element_clear(qc[i]); }
   }
+  /* 2b. products with a pair count per output: segments of 1, 2 and 5 pairs (P[0..7]) in one call,
+   * each against element_prod_pairing of the CPU vtable */
+  {
+    static const size_t off[4] = {0, 1, 3, 8};
+    int l1 = pairing_length_in_bytes_G1(gpu), l2 = pairing_length_in_bytes_G2(gpu), lt = pairing_length_in_bytes_GT(gpu);
+    unsigned char *b1 = malloc((size_t)8 * (l1 + l2) + (size_t)3 * lt), *b2 = b1 + (size_t)8 * l1, *bo = b2 + (size_t)8 * l2;
+    element_t pc[5], qc[5];
+    for (i = 0; i < 8; i++) { element_to_bytes(b1 + (size_t)i * l1, P[i]); element_to_bytes(b2 + (size_t)i * l2, Q[i]); }
+    int rc = pbc_b200_prod_pairing_batch_v(gpu, bo, b1, b2, off, 3);
+    if (rc) { printf("pbc_b200_prod_pairing_batch_v failed\n"); bad++; }
+    for (i = 0; i < 5; i++) { element_init_G1(pc[i], cpu); element_init_G2(qc[i], cpu); }
+    for (int s = 0; s < 3 && !rc; s++) {
+      int len = (int)(off[s + 1] - off[s]);
+      for (i = 0; i < len; i++) { copy_elem(pc[i], P[off[s] + i]); copy_elem(qc[i], Q[off[s] + i]); }
+      element_prod_pairing(e2, pc, qc, len);
+      element_from_bytes(ep, bo + (size_t)s * lt);
+      if (!same(ep, e2)) { printf("pbc_b200_prod_pairing_batch_v mismatch in segment %d\n", s); bad++; }
+    }
+    for (i = 0; i < 5; i++) { element_clear(pc[i]); element_clear(qc[i]); }
+    free(b1);
+  }
   /* 3. pairing_pp_* */
   {
     pairing_pp_t pp;
@@ -118,7 +141,7 @@ int main(int argc, char **argv) {
     for (i = 0; i < m; i++) { element_clear(K[i]); element_clear(R[i]); }
     element_clear(ref); element_clear(kc);
   }
-  printf("shim_test: %s (%d batch pairings, prod, pp, identity, pow_zn; G1 %d B, G2 %d B, GT %d B)\n",
+  printf("shim_test: %s (%d batch pairings, prod, ragged prod 1+2+5, pp, identity, pow_zn; G1 %d B, G2 %d B, GT %d B)\n",
          bad ? "FAILED" : "OK", n, pairing_length_in_bytes_G1(gpu), pairing_length_in_bytes_G2(gpu),
          pairing_length_in_bytes_GT(gpu));
   for (i = 0; i < n; i++) { element_clear(P[i]); element_clear(Q[i]); element_clear(E[i]); }

@@ -237,6 +237,33 @@ int pbc_b200_pairing_length_in_bytes_compressed_G1(const pbc_b200_pairing_t *p);
 int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t *p, unsigned char *out, const unsigned char *in,
                                       size_t n);
 
+/* Batched element_from_hash on G2 (curve_from_hash, ecc/curve.c:455-482, on the twist): out[i] = the
+ * G2 element the reference derives from the `len` bytes at data + i*len.  The twist's field K sets x:
+ * type f (K = F_q^2, fq_from_hash arith/fieldquadratic.c:311-316) hashes x0 from the first len/2 bytes
+ * and x1 from the rest; types d and g (K = F_q^3, F_q^5, polymod_from_hash arith/poly.c:341-348) give
+ * every coefficient the hash of the whole data.  Then x <- x^2 + 1 until x^3 + a'x + b' is a square of K
+ * (zero counts as one in F_q^2, not in F_q^3 / F_q^5, as fq_is_sqr and polymod_is_sqr decide), y its
+ * root with element_sign(y) >= 0 (fq_sign / polymod_sgn on the reference basis).  The twist has no
+ * cofactor (ecc/f_param.c:383, ecc/d_param.c:1057, ecc/g_param.c:1319): the point found is the output
+ * and usually lies outside the order-r subgroup, as in the reference.  Type f needs q = 3 mod 4; types d
+ * and g take any q.  Types a and a1: G2 = G1, the calls give the bytes of pbc_b200_g1_from_hash.  Type e
+ * fails with a message.  len is 1..2^20. */
+int pbc_b200_g2_from_hash(pbc_b200_pairing_t *p, unsigned char *out, const unsigned char *data,
+                          size_t len, size_t n);
+int pbc_b200_g2_from_hash_device(pbc_b200_pairing_t *p, void *d_out, const void *d_data, size_t len,
+                                 size_t n, void *stream);
+
+/* Batched element_from_bytes_compressed on G2 (ecc/curve.c:762-813): each input is x in wire format
+ * (pbc_b200_pairing_length_in_bytes_compressed_G2 - 1 bytes: 40 for f, 60 for d159, 95 for g149, 3 wb
+ * for type d with wb-byte coordinates) followed by one byte; a non-zero byte selects the root y with
+ * element_sign(y) > 0, zero the other one.  Coordinates >= q are reduced mod q, as element_from_bytes
+ * does.  x^3 + a'x + b' = 0 gives (x, 0); an x with no point on the twist gives zero bytes.  Compression
+ * is x || (1 if element_sign(y) > 0 else 0) and needs no GPU; pbc_b200/pairing.py has it.  Types a and a1
+ * as G1, type e fails. */
+int pbc_b200_pairing_length_in_bytes_compressed_G2(const pbc_b200_pairing_t *p);
+int pbc_b200_g2_from_bytes_compressed(pbc_b200_pairing_t *p, unsigned char *out, const unsigned char *in,
+                                      size_t n);
+
 /* Multi-GPU fan-out for the host-buffer entry points: use devices [0, count).  count = 0 means
  * every visible device.  Default is 1 (the current device). */
 int pbc_b200_set_devices(pbc_b200_pairing_t *p, int count);

@@ -55,6 +55,10 @@ lib.pbc_b200_g1_from_hash.argtypes = [_P, _P, _P, C.c_size_t, C.c_size_t]
 lib.pbc_b200_g1_from_hash_device.argtypes = [_P, _P, _P, C.c_size_t, C.c_size_t, _P]
 lib.pbc_b200_pairing_length_in_bytes_compressed_G1.argtypes = [_P]
 lib.pbc_b200_g1_from_bytes_compressed.argtypes = [_P, _P, _P, C.c_size_t]
+lib.pbc_b200_g2_from_hash.argtypes = [_P, _P, _P, C.c_size_t, C.c_size_t]
+lib.pbc_b200_g2_from_hash_device.argtypes = [_P, _P, _P, C.c_size_t, C.c_size_t, _P]
+lib.pbc_b200_pairing_length_in_bytes_compressed_G2.argtypes = [_P]
+lib.pbc_b200_g2_from_bytes_compressed.argtypes = [_P, _P, _P, C.c_size_t]
 lib.pbc_b200_set_devices.argtypes = [_P, C.c_int]
 lib.pbc_b200_host_alloc.argtypes = [C.c_size_t]
 lib.pbc_b200_host_alloc.restype = _P

@@ -52,6 +52,8 @@ void dw_pp_init(const uint8_t*, uint32_t*, size_t, cudaStream_t) {}
 void dw_group(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
 void dw_from_hash(const uint8_t*, int, uint8_t*, size_t, cudaStream_t) {}
 void dw_decompress(const uint8_t*, uint8_t*, size_t, cudaStream_t) {}
+void dw_g2_from_hash(const uint8_t*, int, uint8_t*, size_t, cudaStream_t) {}
+void dw_g2_decompress(const uint8_t*, uint8_t*, size_t, cudaStream_t) {}
 void dw_tower_op(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
 void dw_fq_op(int, uint8_t*, const uint8_t*, const uint8_t*, size_t, cudaStream_t) {}
 }  // namespace pbcb200_dw
@@ -183,6 +185,10 @@ struct pbc_b200_pairing_s {
   ZrConsts zr;
   HashConsts hash;
   bool hash_ok = false;        // element_from_hash available (q = 3 mod 4 or 5 mod 8)
+  // element_from_hash and compressed points on G2 (types f, d, g): square roots in the twist's field K
+  G2HashConsts g2h;
+  G2HashConstsT<pbcb200_dw::kLimbs> dw_g2h;
+  bool g2_hash_ok = false;
   int zr_len = 20;
   int ndev = 1;
   bool profile = false;        // record CUDA events between the kernels of the device-API path
@@ -497,6 +503,50 @@ static void fill_hash(pbc_b200_pairing_s* p, const BigUInt& q, const BigUInt& co
 static void to_mont(uint32_t* out, const BigUInt& x, const BigUInt& q, int n) {
   ((x % q).shl(32 * (size_t)n) % q).to_words(out, n);
 }
+
+// element_from_hash / compressed points on G2 (group_cc.cuh, G2HashConstsT): square roots in K = F_q^k.
+// k = 2 (type f): the norm method over F_q roots z^((q + 1)/4), so q = 3 mod 4; isq is i^2 of the basis
+// in use.  k = 3, 5: Q = q^k = q mod 8 picks t^((Q + 1)/4), Atkin or Tonelli-Shanks; for the last,
+// q^(k-1) + .. + 1 is odd, so Q - 1 = 2^s Qo has the s of q - 1 and c = z^Qo lies in F_q.
+template <int NS>
+static void fill_g2_hash(pbc_b200_pairing_s* p, G2HashConstsT<NS>& c, const BigUInt& q, int k, const BigUInt& isq) {
+  memset(&c, 0, sizeof c);
+  p->g2_hash_ok = false;
+  const BigUInt one(1), two(2), qm1 = q - one;
+  BigUInt leg = qm1 / two, e;
+  leg.to_words(c.leg, 8);
+  c.legbits = (uint32_t)leg.bits();
+  if (k == 2) {
+    if (q.word(0) % 4 != 3) return;
+    e = (q + one) / BigUInt(4);
+    to_mont(c.isq, isq, q, NS);
+    to_mont(c.isq_inv, BigUInt::invmod(isq % q, q), q, NS);
+    c.mode = 1;
+  } else {
+    BigUInt Q = q;
+    for (int i = 1; i < k; i++) Q = Q * q;
+    if (q.word(0) % 4 == 3) { c.mode = 1; e = (Q + one) / BigUInt(4); }
+    else if (q.word(0) % 8 == 5) { c.mode = 2; e = (Q - BigUInt(5)) / BigUInt(8); }
+    else {
+      BigUInt Qo = Q - one, z(2);
+      uint32_t s = 0;
+      while (!Qo.bit(0)) { Qo = Qo / two; s++; }
+      for (int tries = 0; !(BigUInt::powmod(z, leg, q) == qm1); tries++) {
+        if (tries == 200) return;
+        z = z + one;
+      }
+      c.mode = 3;
+      c.ts_s = s;
+      e = (Qo - one) / two;
+      to_mont(c.ts_c, BigUInt::powmod(z, Qo % qm1, q), q, NS);
+      p->derived["g2_sqrt_nonresidue"] = {z};
+    }
+  }
+  if (e.bits() > 32 * 24) return;
+  e.to_words(c.exp, 24);
+  c.expbits = (uint32_t)e.bits();
+  p->g2_hash_ok = true;
+}
 template <int NS>
 static void fill_cc(CCConstsT<NS>* c, const BigUInt& A, const BigUInt& B, const BigUInt& r, const BigUInt& q) {
   memset(c, 0, sizeof *c);
@@ -651,6 +701,7 @@ static int init_type_f(pbc_b200_pairing_s* p, const std::map<std::string, std::s
   c.slots_ok = (c.nice && (q * BigUInt(3)).bits() <= 160 && (q * q * BigUInt(12)).bits() <= 320) ? 1u : 0u;
   to_mont(c.sigma, sigma, q, kNS);
   to_mont(c.sigma_inv, sigma_inv, q, kNS);
+  fill_g2_hash(p, p->g2h, q, 2, B.ok ? q - one : Kref.beta);     // i^2 = -1 internal, beta reference
   for (int j = 1; j < 6; j++) { put2(c.tau[j - 1], taup[j]); put2(c.tau_inv[j - 1], tauinv[j]); }
 
   BigUInt num = (q2 * q2 + one) - q2, te, rem;
@@ -811,6 +862,7 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
     fill_fp_consts(&p->fp, q, kNS);
     fill_cc(&p->cc, a, b, r, q);
     fill_hash(p, q, hco);                  // G1 cofactor = h (ecc/d_param.c:1016)
+    fill_g2_hash(p, p->g2h, q, 3, BigUInt());
     return fill_type_d<kNS>(p, p->d, q, r, a, b, nqr, c0, c1, c2);
   }
   const int NW = pbcb200_dw::kLimbs;
@@ -854,6 +906,7 @@ static int init_type_d(pbc_b200_pairing_s* p, const std::map<std::string, std::s
     }
     p->dw_naf.len = (uint32_t)dg.size();
   }
+  fill_g2_hash(p, p->dw_g2h, q, 3, BigUInt());
   return fill_type_d<NW>(p, p->dw_d, q, r, a, b, nqr, c0, c1, c2);
 }
 
@@ -885,6 +938,7 @@ static int init_type_g(pbc_b200_pairing_s* p, const std::map<std::string, std::s
     if (ith != tab.end()) BigUInt::from_dec(ith->second, &hco);
     fill_hash(p, q, hco);                  // G1 cofactor = h (ecc/g_param.c:1267)
   }
+  fill_g2_hash(p, p->g2h, q, 5, BigUInt());
   GConsts& c = p->g;
   memset(&c, 0, sizeof c);
   BigUInt v = nqr % q, vinv = BigUInt::invmod(v, q), one(1);
@@ -1199,9 +1253,9 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
   std::lock_guard<std::mutex> lk(g_const_mu);
   if (g_const_owner[dev] != p->id && p->dwide) {
     CUDA_OK(cudaDeviceSynchronize());
-    pbcb200_dw::DWideConsts w = {&p->fp, &p->dw_cc, &p->dw_naf, &p->dw_d, &p->dw_zr, &p->hash, &p->dw_x,
+    pbcb200_dw::DWideConsts w = {&p->fp, &p->dw_cc, &p->dw_naf, &p->dw_d, &p->dw_zr, &p->hash, &p->dw_x, &p->dw_g2h,
                                  sizeof p->fp, sizeof p->dw_cc, sizeof p->dw_naf, sizeof p->dw_d, sizeof p->dw_zr,
-                                 sizeof p->hash, sizeof p->dw_x};
+                                 sizeof p->hash, sizeof p->dw_x, sizeof p->dw_g2h};
     const int e = pbcb200_dw::dw_upload(w);
     if (e == -2) return fail("type d: this build has no eight-limb instance (160..255-bit q)");
     if (e < 0) return fail("type d: the constants of the eight-limb instance do not match its layout");
@@ -1241,6 +1295,7 @@ static int ctx_prepare(pbc_b200_pairing_s* p, int dev) {
     if (p->type == 'f') CUDA_OK(cudaMemcpyToSymbol(c_f, &p->f, sizeof(FConsts)));
     if (p->type == 'd') CUDA_OK(cudaMemcpyToSymbol(c_d, &p->d, sizeof(DConsts)));
     if (p->type == 'g') CUDA_OK(cudaMemcpyToSymbol(c_g, &p->g, sizeof(GConsts)));
+    if (p->type == 'f' || p->type == 'd' || p->type == 'g') CUDA_OK(cudaMemcpyToSymbol(c_g2h, &p->g2h, sizeof(G2HashConsts)));
     CUDA_OK(cudaDeviceSynchronize());
     g_const_owner[dev] = p->id;
   }
@@ -2364,12 +2419,17 @@ int pbc_b200_gt_pow_zn_device(pbc_b200_pairing_t* p, void* d_out, const void* d_
 }
 
 
-// element_from_hash on G1 (include/pbc_field.h:202-212 -> ecc/curve.c:455-482), batched
+// types f, d, g: G2 is the twist, with kernels of its own; types a and a1: G2 = G1
+static bool g2_is_twist(const pbc_b200_pairing_s* p) { return p->type == 'f' || p->type == 'd' || p->type == 'g'; }
+
+// element_from_hash on G1 or G2 (include/pbc_field.h:202-212 -> ecc/curve.c:455-482), batched
 static int run_from_hash(pbc_b200_pairing_s* p, unsigned char* out, const unsigned char* data, size_t len, size_t n,
-                         bool device, void* stream) {
+                         bool device, void* stream, bool g2 = false) {
   if (!p || (n && (!out || !data))) return fail("null argument");
   if (p->type == 'e') return fail("element_from_hash: not available for type e (q = 1 mod 16 needs a 34-limb Tonelli-Shanks)");
-  if (p->type != '1' && !p->hash_ok) return fail("element_from_hash: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q) and a cofactor below 2^384");
+  const bool twist = g2 && g2_is_twist(p);
+  if (twist && !p->g2_hash_ok) return fail("element_from_hash on G2: needs square roots in the twist's field (type f: q = 3 mod 4)");
+  if (!twist && p->type != '1' && !p->hash_ok) return fail("element_from_hash: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q) and a cofactor below 2^384");
   if (len == 0 || len > (1u << 20)) return fail("element_from_hash: hash length must be 1..2^20 bytes");
   if (n == 0) return 0;
   std::lock_guard<std::mutex> lk(p->mu);
@@ -2379,7 +2439,7 @@ static int run_from_hash(pbc_b200_pairing_s* p, unsigned char* out, const unsign
   if (!device) dev_lock.lock();
   if (ctx_prepare(p, dev)) return 1;
   DevCtx& c = p->ctx[dev];
-  size_t elen = (size_t)p->g1_len;
+  size_t elen = twist ? (size_t)p->g2_len : (size_t)p->g1_len;
   size_t wsb = p->type == 'a' ? n * 64 * (2 + 1 + 1) : 16;
   if (p->type == '1') wsb = n * kSlotA1 * (2 + 1 + 1);
   size_t stage = device ? 0 : n * (elen + len);
@@ -2423,6 +2483,13 @@ static int run_from_hash(pbc_b200_pairing_s* p, unsigned char* out, const unsign
     unsigned gf = (unsigned)((n + kBlockFinal - 1) / kBlockFinal);
     k_a_g1_finish<kBlockFinal><<<gf, kBlockFinal, (size_t)4 * 64 * kBlockFinal, st>>>(xyz, zarr, d_out, n);
     LAUNCHED();
+  } else if (twist) {
+    unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
+    if (p->dwide) pbcb200_dw::dw_g2_from_hash(d_data, (int)len, d_out, n, st);
+    else if (p->type == 'f') k_cc_g2_from_hash<KF2, kBlockCC><<<g, kBlockCC, 0, st>>>(d_data, (int)len, d_out, n);
+    else if (p->type == 'g') k_cc_g2_from_hash<KF5, kBlockCC><<<g, kBlockCC, 0, st>>>(d_data, (int)len, d_out, n);
+    else k_cc_g2_from_hash<KF3, kBlockCC><<<g, kBlockCC, 0, st>>>(d_data, (int)len, d_out, n);
+    LAUNCHED();
   } else {
     unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
     if (p->dwide) pbcb200_dw::dw_from_hash(d_data, (int)len, d_out, n, st);
@@ -2447,16 +2514,23 @@ int pbc_b200_g1_from_hash_device(pbc_b200_pairing_t* p, void* d_out, const void*
                                  void* stream) {
   return run_from_hash(p, (unsigned char*)d_out, (const unsigned char*)d_data, len, n, true, stream);
 }
+int pbc_b200_g2_from_hash(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* data, size_t len, size_t n) {
+  return run_from_hash(p, out, data, len, n, false, nullptr, true);
+}
+int pbc_b200_g2_from_hash_device(pbc_b200_pairing_t* p, void* d_out, const void* d_data, size_t len, size_t n,
+                                 void* stream) {
+  return run_from_hash(p, (unsigned char*)d_out, (const unsigned char*)d_data, len, n, true, stream, true);
+}
 }
 
 
-// element_from_bytes_compressed on G1 (ecc/curve.c:799-813), batched; host buffers
-extern "C" int pbc_b200_pairing_length_in_bytes_compressed_G1(const pbc_b200_pairing_t* p) { return p->g1_len / 2 + 1; }
-extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in,
-                                                 size_t n) {
+// element_from_bytes_compressed on G1 or G2 (ecc/curve.c:799-813), batched; host buffers
+static int run_decompress(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in, size_t n, bool g2) {
   if (!p || (n && (!out || !in))) return fail("null argument");
   if (p->type == 'e') return fail("element_from_bytes_compressed: not available for type e");
-  if (p->type != '1' && !p->hash_ok) return fail("element_from_bytes_compressed: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q)");
+  const bool twist = g2 && g2_is_twist(p);
+  if (twist && !p->g2_hash_ok) return fail("element_from_bytes_compressed on G2: needs square roots in the twist's field (type f: q = 3 mod 4)");
+  if (!twist && p->type != '1' && !p->hash_ok) return fail("element_from_bytes_compressed: needs q = 3 mod 4 or q = 5 mod 8 (or type d with 160..255-bit q)");
   if (n == 0) return 0;
   std::lock_guard<std::mutex> lk(p->mu);
   int dev = 0;
@@ -2464,7 +2538,7 @@ extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned
   std::lock_guard<std::mutex> dev_lock(g_dev_mu[dev & 63]);
   if (ctx_prepare(p, dev)) return 1;
   DevCtx& c = p->ctx[dev];
-  size_t clen = (size_t)p->g1_len / 2 + 1, elen = (size_t)p->g1_len, need = n * (clen + elen) + 16;
+  size_t elen = twist ? (size_t)p->g2_len : (size_t)p->g1_len, clen = elen / 2 + 1, need = n * (clen + elen) + 16;
   if (c.cap_dev < need) {
     CUDA_OK(cudaDeviceSynchronize());
     cudaFree(c.ws_dev);
@@ -2483,6 +2557,12 @@ extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned
   } else if (p->type == 'a') {
     unsigned g = (unsigned)((n + kBlockMiller - 1) / kBlockMiller);
     k_a_g1_decompress<kBlockMiller><<<g, kBlockMiller, (size_t)5 * 64 * kBlockMiller, st>>>(d_in, d_out, n);
+  } else if (twist) {
+    unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
+    if (p->dwide) pbcb200_dw::dw_g2_decompress(d_in, d_out, n, st);
+    else if (p->type == 'f') k_cc_g2_decompress<KF2, kBlockCC><<<g, kBlockCC, 0, st>>>(d_in, d_out, n);
+    else if (p->type == 'g') k_cc_g2_decompress<KF5, kBlockCC><<<g, kBlockCC, 0, st>>>(d_in, d_out, n);
+    else k_cc_g2_decompress<KF3, kBlockCC><<<g, kBlockCC, 0, st>>>(d_in, d_out, n);
   } else {
     unsigned g = (unsigned)((n + kBlockCC - 1) / kBlockCC);
     if (p->dwide) pbcb200_dw::dw_decompress(d_in, d_out, n, st);
@@ -2494,6 +2574,17 @@ extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned
   CUDA_OK(cudaMemcpyAsync(out, d_out, n * elen, cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   return 0;
+}
+extern "C" int pbc_b200_pairing_length_in_bytes_compressed_G1(const pbc_b200_pairing_t* p) { return p->g1_len / 2 + 1; }
+extern "C" int pbc_b200_g1_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in,
+                                                 size_t n) {
+  return run_decompress(p, out, in, n, false);
+}
+// the x of the twist point (types f, d, g) or of the G1 point (a, a1) and one sign byte
+extern "C" int pbc_b200_pairing_length_in_bytes_compressed_G2(const pbc_b200_pairing_t* p) { return p->g2_len / 2 + 1; }
+extern "C" int pbc_b200_g2_from_bytes_compressed(pbc_b200_pairing_t* p, unsigned char* out, const unsigned char* in,
+                                                 size_t n) {
+  return run_decompress(p, out, in, n, true);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -34,7 +34,7 @@ static unsigned grid(size_t n, int block) { return (unsigned)((n + block - 1) / 
 int dw_upload(const DWideConsts& c) {
   if (c.fp_bytes != sizeof(FpConsts) || c.cc_bytes != sizeof(CCConsts) || c.naf_bytes != sizeof(CCNaf) ||
       c.d_bytes != sizeof(DConsts) || c.zr_bytes != sizeof(ZrConsts) || c.hash_bytes != sizeof(HashConsts) ||
-      c.x_bytes != sizeof(FqWideConstsT<kNS>))
+      c.x_bytes != sizeof(FqWideConstsT<kNS>) || c.g2h_bytes != sizeof(G2HashConsts))
     return -1;
   cudaError_t e;
   if ((e = cudaMemcpyToSymbol(c_fp, c.fp, c.fp_bytes)) != cudaSuccess) return e;
@@ -43,6 +43,7 @@ int dw_upload(const DWideConsts& c) {
   if ((e = cudaMemcpyToSymbol(c_d, c.d, c.d_bytes)) != cudaSuccess) return e;
   if ((e = cudaMemcpyToSymbol(c_zr, c.zr, c.zr_bytes)) != cudaSuccess) return e;
   if ((e = cudaMemcpyToSymbol(c_hash, c.hash, c.hash_bytes)) != cudaSuccess) return e;
+  if ((e = cudaMemcpyToSymbol(c_g2h, c.g2h, c.g2h_bytes)) != cudaSuccess) return e;
   return (int)cudaMemcpyToSymbol(c_fqx, c.x, c.x_bytes);
 }
 
@@ -75,6 +76,12 @@ void dw_from_hash(const uint8_t* data, int len, uint8_t* out, size_t n, cudaStre
 }
 void dw_decompress(const uint8_t* in, uint8_t* out, size_t n, cudaStream_t st) {
   k_cc_g1_decompress<kBlockW, 0><<<grid(n, kBlockW), kBlockW, 0, st>>>(in, out, n);
+}
+void dw_g2_from_hash(const uint8_t* data, int len, uint8_t* out, size_t n, cudaStream_t st) {
+  k_cc_g2_from_hash<KF3, kBlockW><<<grid(n, kBlockW), kBlockW, 0, st>>>(data, len, out, n);
+}
+void dw_g2_decompress(const uint8_t* in, uint8_t* out, size_t n, cudaStream_t st) {
+  k_cc_g2_decompress<KF3, kBlockW><<<grid(n, kBlockW), kBlockW, 0, st>>>(in, out, n);
 }
 void dw_tower_op(int op, uint8_t* out, const uint8_t* a, const uint8_t* b, size_t n, cudaStream_t st) {
   k_d_tower_op<<<grid(n, 64), 64, 0, st>>>(op, out, a, b, n);

@@ -317,6 +317,196 @@ k_cc_g1_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, si
 // field: struct El; mul/sqr/inv on pointers (the tower's out-of-line routines), add/sub/dbl inline,
 // wire <-> basis-in-use conversion, and the curve constants.
 // ---------------------------------------------------------------------------------------------
+
+// element_from_hash and compressed points on G2 (curve_from_hash / element_from_bytes_compressed on the
+// twist): the square-root data of K, derived at init (engine.cu, fill_g2_hash)
+template <int NS>
+struct G2HashConstsT {
+  uint32_t exp[24];      // type f: (q + 1)/4, roots in F_q.  Types d, g (Q = q^k, k odd): mode 1 (Q + 1)/4,
+                         // mode 2 (Q - 5)/8 (Atkin), mode 3 (Qo - 1)/2 with Q - 1 = 2^s Qo (Tonelli-Shanks)
+  uint32_t leg[8];       // (q - 1)/2: the Legendre symbol of a norm
+  uint32_t expbits, legbits, mode, ts_s;
+  uint32_t ts_c[NS];     // mode 3: z^Qo for a non-residue z of F_q (it lies in F_q), Montgomery form
+  uint32_t isq[NS];      // type f: i^2 of the basis in use (-1 internal, beta reference), Montgomery form
+  uint32_t isq_inv[NS];
+};
+typedef G2HashConstsT<kNS> G2HashConsts;
+__constant__ G2HashConsts c_g2h;
+
+// a^e, e a plain little-endian exponent of `bits` bits (a^0 = 1)
+__device__ __noinline__ void fq_pow_words(Fq* r, const Fq* a, const uint32_t* e, int bits) {
+  Fq x = *a, acc = *a;
+  for (int j = bits - 2; j >= 0; j--) {
+    fq_sqr(acc, acc);
+    if ((e[j >> 5] >> (j & 31)) & 1u) fq_mul(acc, acc, x);
+  }
+  if (bits == 0) fq_one(acc);
+  *r = acc;
+}
+// n^((q - 1)/2) == 1: n is a non-zero square of F_q.  The helpers below whose locals have their
+// address taken are out of line with those locals at function scope: inlined into the G2 kernels, such
+// a local of KF5::is_sqr was seen to share its stack slot with the kernel's live t (stack discipline
+// note in pairing_f.cuh)
+__device__ __noinline__ bool fq_is_nonzero_sqr(Fq n) {
+  Fq l, one;
+  fq_pow_words(&l, &n, c_g2h.leg, (int)c_g2h.legbits);
+  fq_one(one);
+  return fq_eq(l, one);
+}
+// fp_sgn_odd (arith/montfp.c:460-472): 0 for zero, 1 for an odd canonical residue, -1 for an even one
+__device__ __forceinline__ int fq_sgn(const Fq& a) {
+  uint32_t c[kNS], o1[kNS] = {1};
+  mont_mul_ps<kNS, false>(c, a.v, o1);
+  if (fp_is_zero<kNS>(c)) return 0;
+  return (c[0] & 1u) ? 1 : -1;
+}
+// K^* of odd degree k has a square root method by q mod 8 (Q = q^k = q mod 8); t a non-zero square
+// (out of line, locals at function scope: the stack discipline note in pairing_f.cuh)
+template <class KF>
+__device__ __noinline__ void kf_pow(typename KF::El* r, const typename KF::El* a, const uint32_t* e, int bits) {
+  typename KF::El x = *a, acc = *a;
+  for (int j = bits - 2; j >= 0; j--) {
+    KF::sqr(&acc, &acc);
+    if ((e[j >> 5] >> (j & 31)) & 1u) KF::mul(&acc, &acc, &x);
+  }
+  if (bits == 0) KF::one(acc);
+  *r = acc;
+}
+template <class KF>
+__device__ __noinline__ void kf_sqrt_odd(typename KF::El* yp, const typename KF::El* tp) {
+  typedef typename KF::El El;
+  El y, t = *tp, b, w, u, one;
+  const int mode = (int)c_g2h.mode, bits = (int)c_g2h.expbits;
+  if (mode == 1) {                       // t^((Q + 1)/4)
+    kf_pow<KF>(yp, &t, c_g2h.exp, bits);
+    return;
+  }
+  if (mode == 2) {                       // Atkin: b = (2t)^((Q - 5)/8), i = 2 t b^2, root = t b (i - 1)
+    KF::add(u, t, t);
+    kf_pow<KF>(&b, &u, c_g2h.exp, bits);
+    KF::sqr(&w, &b);
+    KF::mul(&w, &w, &u);
+    KF::one(one);
+    KF::sub(w, w, one);
+    KF::mul(&y, &t, &b);
+    KF::mul(yp, &y, &w);
+    return;
+  }
+  // Tonelli-Shanks: x = t^((Qo - 1)/2), y = t x, b = y x = t^Qo.  q^(k-1) + .. + q + 1 is odd, so the
+  // 2-Sylow subgroup of K^* is that of F_q^*: b, c and every w below lie in F_q (coefficient 0)
+  kf_pow<KF>(&w, &t, c_g2h.exp, bits);
+  KF::mul(&y, &t, &w);
+  KF::mul(&b, &y, &w);
+  Fq bq = b.c[0], c, wq, fone;
+  fq_set(c, c_g2h.ts_c);
+  fq_one(fone);
+  int m = (int)c_g2h.ts_s;
+  for (int it = 0; it < 64 && !fq_eq(bq, fone); it++) {
+    int i = 1;
+    fq_sqr(wq, bq);
+    while (i < m && !fq_eq(wq, fone)) { fq_sqr(wq, wq); i++; }
+    if (i >= m) break;
+    wq = c;
+    for (int j = 0; j < m - i - 1; j++) fq_sqr(wq, wq);
+    KF::scale(y, y, wq);
+    fq_sqr(c, wq);
+    fq_mul(bq, bq, c);
+    m = i;
+  }
+  *yp = y;
+}
+
+#if !PBC_FQ_WIDE
+// F_q^2 = F_q[i]/(i^2 - isq): x0 + x1 i is a square iff its norm x0^2 - isq x1^2 is one in F_q, zero
+// included (fq_is_sqr, arith/fieldquadratic.c:339-355)
+__device__ __noinline__ bool f2_is_sqr(const F2* t) {
+  Fq n, u, k;
+  fq_sqr(n, t->a);
+  fq_sqr(u, t->b);
+  fq_set(k, c_g2h.isq);
+  fq_mul(u, u, k);
+  fq_sub(n, n, u);
+  return fq_is_zero(n) || fq_is_nonzero_sqr(n);
+}
+// a root of the square t, the norm method of fq_sqrt (arith/fieldquadratic.c:357-391):  m = sqrt(N(t)),
+// z = (x0 +- m)/2 whichever is a square, y0 = sqrt(z), y1 = x1 / (2 y0).  x1 = 0 separately: then the root
+// is sqrt(x0) or sqrt(x0 / isq) i.  F_q roots are z^((q + 1)/4) (q = 3 mod 4).
+__device__ __noinline__ void f2_sqrt(F2* r, const F2* tp) {
+  const F2 t = *tp;
+  const int eb = (int)c_g2h.expbits;
+  Fq n, m, z, y0, u, k;
+  if (fq_is_zero(t.b)) {
+    fq_pow_words(&y0, &t.a, c_g2h.exp, eb);
+    fq_sqr(u, y0);
+    if (fq_eq(u, t.a)) { r->a = y0; fq_zero(r->b); return; }
+    fq_set(k, c_g2h.isq_inv);
+    fq_mul(u, t.a, k);
+    fq_pow_words(&r->b, &u, c_g2h.exp, eb);
+    fq_zero(r->a);
+    return;
+  }
+  fq_sqr(n, t.a);
+  fq_sqr(u, t.b);
+  fq_set(k, c_g2h.isq);
+  fq_mul(u, u, k);
+  fq_sub(n, n, u);
+  fq_pow_words(&m, &n, c_g2h.exp, eb);
+  fq_add(z, t.a, m);
+  fq_halve(z, z);
+  fq_pow_words(&y0, &z, c_g2h.exp, eb);
+  fq_sqr(u, y0);
+  if (!fq_eq(u, z)) {
+    fq_sub(z, z, m);
+    fq_pow_words(&y0, &z, c_g2h.exp, eb);
+  }
+  fq_dbl(u, y0);
+  fq_inv(&u, &u);
+  fq_mul(r->b, t.b, u);
+  r->a = y0;
+}
+// N(x) = x x^q x^(q^2) x^(q^3) x^(q^4) in F_q^5 (as f5_inv)
+__device__ __noinline__ void f5_norm(Fq* n, const F5* x) {
+  F5 f1, f2, t;
+  f5_frob(&f1, x);
+  f5_frob(&f2, &f1);
+  f5_mul(&t, &f1, &f2);
+  f5_frob(&f1, &f2);
+  f5_mul(&t, &t, &f1);
+  f5_frob(&f2, &f1);
+  f5_mul(&t, &t, &f2);
+  f5_mul(&f1, &t, x);
+  *n = f1.c[0];
+}
+__device__ __noinline__ bool f5_is_sqr(const F5* t) {
+  Fq n;
+  f5_norm(&n, t);
+  return fq_is_nonzero_sqr(n);
+}
+#endif
+// N(x) = x x^q x^(q^2) (coefficient 0 of the product; the others are zero)
+__device__ __noinline__ void f3_norm(Fq* n, const F3* x) {
+  F3 t, u;
+  f3_frob(t, *x);
+  f3_frob(u, t);
+  f3_mul(&t, &t, &u);
+  f3_mul(&u, &t, x);
+  *n = u.c[0];
+}
+__device__ __noinline__ bool f3_is_sqr(const F3* t) {
+  Fq n;
+  f3_norm(&n, t);
+  return fq_is_nonzero_sqr(n);
+}
+// polymod_sgn (arith/poly.c:1189-1199) on the reference basis: the first non-zero coefficient
+__device__ __noinline__ int f3_sgn_ref(const F3* y) {
+  F3 o = *y;
+  f3_to_reference(o);
+  int s = fq_sgn(o.c[0]);
+  if (!s) s = fq_sgn(o.c[1]);
+  if (!s) s = fq_sgn(o.c[2]);
+  return s;
+}
+
 #if !PBC_FQ_WIDE
 struct KF2 {                       // type f
   typedef F2 El;
@@ -351,7 +541,47 @@ struct KF2 {                       // type f
     fq_to_wire(p, o.a);
     fq_to_wire(p + kWS, o.b);
   }
+  // element_from_hash, compressed points
+  static __device__ __forceinline__ void from_wire_b(El& r, const uint8_t* p) {    // no alignment needed
+    Fq s;
+    fq_from_wire_b<kWS>(r.a, p);
+    fq_from_wire_b<kWS>(r.b, p + kWS);
+    fq_set(s, c_f.sigma);
+    fq_mul(r.b, r.b, s);
+  }
+  // fq_from_hash (arith/fieldquadratic.c:311-316): x0 from the first len/2 bytes, x1 from the rest
+  static __device__ __forceinline__ void from_hash(El& r, const uint8_t* data, int len) {
+    uint32_t w[kNS];
+    Fq s;
+    const int k = len / 2;
+    hash_to_words<kNS>(w, data, k);
+    fq_set(r.a, w);
+    hash_to_words<kNS>(w, data + k, len - k);
+    fq_set(r.b, w);
+    fq_set(s, c_fp.r2);
+    fq_mul(r.a, r.a, s);
+    fq_mul(r.b, r.b, s);
+    fq_set(s, c_f.sigma);
+    fq_mul(r.b, r.b, s);
+  }
+  static __device__ __forceinline__ bool is_sqr(const El& t) { return f2_is_sqr(&t); }
+  static __device__ __forceinline__ void sqrt(El& r, const El& t) { f2_sqrt(&r, &t); }
+  static __device__ __forceinline__ void neg(El& r, const El& a) { f2_neg(r, a); }
+  // fq_sign (arith/fieldquadratic.c:159-165) on the reference basis: x1 = sigma^-1 times the one in use
+  static __device__ __forceinline__ int sign(const El& y) {
+    int s = fq_sgn(y.a);
+    if (s) return s;
+    Fq k, b;
+    fq_set(k, c_f.sigma_inv);
+    fq_mul(b, y.b, k);
+    return fq_sgn(b);
+  }
 };
+#endif
+#if PBC_FQ_WIDE
+constexpr int kWB3 = 0;            // the run-time width
+#else
+constexpr int kWB3 = kWS;
 #endif
 struct KF3 {                       // type d
   typedef F3 El;
@@ -380,6 +610,30 @@ struct KF3 {                       // type d
 #pragma unroll
     for (int i = 0; i < 3; i++) fq_to_wire(p + i * fq_wb(), o.c[i]);
   }
+  // element_from_hash, compressed points
+  static __device__ __forceinline__ void from_wire_b(El& r, const uint8_t* p) {    // no alignment needed
+#pragma unroll
+    for (int i = 0; i < 3; i++) fq_from_wire_b<kWB3>(r.c[i], p + i * fq_wb());
+    f3_to_internal(r);
+  }
+  // polymod_from_hash (arith/poly.c:341-348): every coefficient is the hash of the whole data
+  static __device__ __forceinline__ void from_hash(El& r, const uint8_t* data, int len) {
+    uint32_t w[kNS];
+    Fq s;
+    hash_to_words<kNS>(w, data, len);
+    fq_set(r.c[0], w);
+    fq_set(s, c_fp.r2);
+    fq_mul(r.c[0], r.c[0], s);
+    r.c[1] = r.c[0];
+    r.c[2] = r.c[0];
+    f3_to_internal(r);
+  }
+  // polymod_is_sqr (arith/poly.c:617-632): t^((Q - 1)/2) == 1 = N(t)^((q - 1)/2) == 1; zero is not a square
+  static __device__ __forceinline__ bool is_sqr(const El& t) { return f3_is_sqr(&t); }
+  static __device__ __forceinline__ void sqrt(El& r, const El& t) { kf_sqrt_odd<KF3>(&r, &t); }
+  static __device__ __forceinline__ void scale(El& r, const El& a, const Fq& k) { f3_scale(r, a, k); }
+  static __device__ __forceinline__ void neg(El& r, const El& a) { f3_neg(r, a); }
+  static __device__ __forceinline__ int sign(const El& y) { return f3_sgn_ref(&y); }
 };
 
 #if !PBC_FQ_WIDE
@@ -412,6 +666,28 @@ struct KF5 {                       // type g (19-byte coordinates)
     if (zero) f5_zero(o);
 #pragma unroll 1
     for (int i = 0; i < 5; i++) fq_to_wire_b<kWG>(p + i * kWG, o.c[i]);
+  }
+  // element_from_hash, compressed points (the reference basis is the one in use)
+  static __device__ __forceinline__ void from_wire_b(El& r, const uint8_t* p) { from_wire(r, p); }
+  static __device__ __forceinline__ void from_hash(El& r, const uint8_t* data, int len) {
+    uint32_t w[kNS];
+    Fq s;
+    hash_to_words<kNS>(w, data, len);
+    fq_set(r.c[0], w);
+    fq_set(s, c_fp.r2);
+    fq_mul(r.c[0], r.c[0], s);
+#pragma unroll
+    for (int i = 1; i < 5; i++) r.c[i] = r.c[0];
+  }
+  static __device__ __forceinline__ bool is_sqr(const El& t) { return f5_is_sqr(&t); }
+  static __device__ __forceinline__ void sqrt(El& r, const El& t) { kf_sqrt_odd<KF5>(&r, &t); }
+  static __device__ __forceinline__ void scale(El& r, const El& a, const Fq& k) { f5_scale(r, a, k); }
+  static __device__ __forceinline__ void neg(El& r, const El& a) { f5_neg(r, a); }
+  static __device__ __forceinline__ int sign(const El& y) {
+    int s = 0;
+#pragma unroll 1
+    for (int i = 0; i < 5 && !s; i++) s = fq_sgn(y.c[i]);
+    return s;
   }
 };
 
@@ -506,6 +782,64 @@ k_cc_g2_mul(const uint8_t* __restrict__ P, const uint8_t* __restrict__ K, uint8_
   KF::mul(&Y, &Y, &u);
   KF::to_wire(out + idx * (2 * KF::wire()), X, inf);
   KF::to_wire(out + idx * (2 * KF::wire()) + KF::wire(), Y, inf);
+}
+
+// element_from_hash on G2 (curve_from_hash, ecc/curve.c:455-482, on the twist): x from the hash, then
+// x <- x^2 + 1 until x^3 + a' x + b' is a square (at most 64 tries, as on G1), y its root with
+// sign(y) >= 0.  The twist has no cofactor (ecc/f_param.c:383, d_param.c:1057, g_param.c:1319): the point
+// found is the output, usually outside the order-r subgroup.
+template <class KF, int BLOCK>
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
+k_cc_g2_from_hash(const uint8_t* __restrict__ data, int len, uint8_t* __restrict__ out, size_t n) {
+  typedef typename KF::El El;
+  size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
+  if (idx >= n) return;
+  El x, y, t, one;
+  KF::from_hash(x, data + idx * (size_t)len, len);
+  KF::one(one);
+  for (int tries = 0; tries < 64; tries++) {
+    KF::sqr(&t, &x);
+    KF::add_curve_a(t);
+    KF::mul(&t, &t, &x);
+    KF::add_curve_b(t);
+    if (KF::is_sqr(t)) break;
+    KF::sqr(&x, &x);
+    KF::add(x, x, one);
+  }
+  KF::sqrt(y, t);
+  if (KF::sign(y) < 0) KF::neg(y, y);
+  KF::to_wire(out + idx * (2 * KF::wire()), x, false);
+  KF::to_wire(out + idx * (2 * KF::wire()) + KF::wire(), y, false);
+}
+
+// element_from_bytes_compressed on G2 (ecc/curve.c:799-813): x || sign byte -> x || y, y the root with
+// sign > 0 for a non-zero byte and the other one for zero.  x^3 + a' x + b' = 0 gives (x, 0); no root
+// gives zero bytes.
+template <class KF, int BLOCK>
+__global__ void __launch_bounds__(BLOCK, kCCMinBlocks)
+k_cc_g2_decompress(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, size_t n) {
+  typedef typename KF::El El;
+  size_t idx = (size_t)blockIdx.x * BLOCK + threadIdx.x;
+  if (idx >= n) return;
+  const uint8_t* p = in + idx * (size_t)(KF::wire() + 1);
+  El x, y, t;
+  KF::from_wire_b(x, p);               // items are wire + 1 bytes apart: byte loads
+  KF::sqr(&t, &x);
+  KF::add_curve_a(t);
+  KF::mul(&t, &t, &x);
+  KF::add_curve_b(t);
+  bool ok = true;
+  y = El();
+  if (!KF::is_zero(t)) {
+    ok = KF::is_sqr(t);
+    if (ok) {
+      KF::sqrt(y, t);
+      const int s = KF::sign(y);
+      if (p[KF::wire()] ? s < 0 : s > 0) KF::neg(y, y);
+    }
+  }
+  KF::to_wire(out + idx * (2 * KF::wire()), x, !ok);
+  KF::to_wire(out + idx * (2 * KF::wire()) + KF::wire(), y, !ok);
 }
 
 #if !PBC_FQ_WIDE

@@ -222,6 +222,56 @@ class Pairing:
             raise PairingError(last_error())
         return out.raw[:n * self.g1_len]
 
+    def g2_from_hash(self, data: bytes, length: int, n=None) -> bytes:
+        """element_from_hash on G2 for n hashes of `length` bytes each, back to back (types f, d, g: the
+        twist point the reference finds, no cofactor; types a, a1: as g1_from_hash)"""
+        if n is None:
+            n = len(data) // length
+        self._need(data, n * length, "g2_from_hash data")
+        out = C.create_string_buffer(max(1, n * self.g2_len))
+        if lib.pbc_b200_g2_from_hash(self._h, C.addressof(out), _addr(data), length, n):
+            raise PairingError(last_error())
+        return out.raw[:n * self.g2_len]
+
+    def g2_from_hash_device(self, d_out, d_data, length, n, stream=0):
+        if lib.pbc_b200_g2_from_hash_device(self._h, d_out, d_data, length, n, stream):
+            raise PairingError(last_error())
+
+    @staticmethod
+    def _sign(coords, wb):
+        """element_sign of a wire-format field element: the parity of its first non-zero coordinate
+        (fp_sgn_odd, fq_sign, polymod_sgn), 1 odd, -1 even, 0 for zero"""
+        for i in range(0, len(coords), wb):
+            v = int.from_bytes(coords[i:i + wb], "big")
+            if v:
+                return 1 if v & 1 else -1
+        return 0
+
+    def g2_compress(self, points: bytes, n=None) -> bytes:
+        """element_to_bytes_compressed on G2 (ecc/curve.c:762-775): x || (1 if sign(y) > 0 else 0), with
+        the sign of the twist's field (the first non-zero coordinate of y decides); host only"""
+        if self.type in ("a", "a1"):
+            return self.g1_compress(points, n)
+        if self.type not in ("f", "d", "g"):
+            raise PairingError("element_to_bytes_compressed: not available for type %s" % self.type)
+        L = self.g2_len
+        if n is None:
+            n = len(points) // L
+        wb = {"f": L // 4, "d": L // 6, "g": L // 10}[self.type]
+        return b"".join(points[i * L:i * L + L // 2] +
+                        bytes([1 if self._sign(points[i * L + L // 2:(i + 1) * L], wb) > 0 else 0]) for i in range(n))
+
+    def g2_decompress(self, data: bytes, n=None) -> bytes:
+        """element_from_bytes_compressed on G2, on the GPU"""
+        clen = lib.pbc_b200_pairing_length_in_bytes_compressed_G2(self._h)
+        if n is None:
+            n = len(data) // clen
+        self._need(data, n * clen, "g2_decompress data")
+        out = C.create_string_buffer(max(1, n * self.g2_len))
+        if lib.pbc_b200_g2_from_bytes_compressed(self._h, C.addressof(out), _addr(data), n):
+            raise PairingError(last_error())
+        return out.raw[:n * self.g2_len]
+
     def g2_pow_zn(self, points: bytes, scalars: bytes, n=None) -> bytes:
         if n is None:
             n = len(points) // self.g2_len

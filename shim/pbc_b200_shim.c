@@ -244,3 +244,28 @@ void element_pow_zn_batch(element_t out[], element_t in[], element_t k[], int n)
   }
   pbc_free(bi);
 }
+
+/* out[i] = element_from_hash(out[i], data + i*len, len) (include/pbc_field.h:202-212 -> curve_from_hash,
+ * ecc/curve.c:455-482) for arrays of G1 or G2 elements of an attached pairing: one GPU batch of n hashes
+ * of len bytes each, back to back.  A G1 hash whose cofactor multiple is the point at infinity comes back
+ * as zero bytes and is set to the identity. */
+void element_from_hash_batch(element_t out[], const void *data, int len, int n) {
+  if (n <= 0) return;
+  pairing_ptr pairing = out[0]->field->pairing;
+  struct attach_s *a = find_attach(pairing);
+  int is_g1 = out[0]->field == pairing->G1;
+  if (!is_g1 && out[0]->field != pairing->G2) pbc_die("pbc_b200: element_from_hash_batch takes G1 or G2 elements");
+  if (len <= 0) pbc_die("pbc_b200: element_from_hash_batch needs len > 0");
+  size_t elen = is_g1 ? a->g1_len : a->g2_len, k;
+  unsigned char *bo = pbc_malloc(elen * (size_t)n);
+  int i;
+  check((is_g1 ? pbc_b200_g1_from_hash : pbc_b200_g2_from_hash)(a->h, bo, data, (size_t)len, (size_t)n),
+        "element_from_hash_batch");
+  for (i = 0; i < n; i++) {
+    const unsigned char *e = bo + (size_t)i * elen;
+    for (k = 0; k < elen && !e[k]; k++) {}
+    if (k == elen) element_set0(out[i]);
+    else element_from_bytes(out[i], (unsigned char *)e);
+  }
+  pbc_free(bo);
+}

@@ -15,6 +15,7 @@
 
 void element_pairing_batch(element_t out[], element_t in1[], element_t in2[], int n);
 void element_pow_zn_batch(element_t out[], element_t in[], element_t k[], int n);
+void element_from_hash_batch(element_t out[], const void *data, int len, int n);
 int pbc_b200_pairing_batch(pairing_t pairing, unsigned char *out, const unsigned char *in1,
                            const unsigned char *in2, size_t n);
 int pbc_b200_prod_pairing_batch_v(pairing_t pairing, unsigned char *out, const unsigned char *in1,
@@ -141,7 +142,29 @@ int main(int argc, char **argv) {
     for (i = 0; i < m; i++) { element_clear(K[i]); element_clear(R[i]); }
     element_clear(ref); element_clear(kc);
   }
-  printf("shim_test: %s (%d batch pairings, prod, ragged prod 1+2+5, pp, identity, pow_zn; G1 %d B, G2 %d B, GT %d B)\n",
+  {  /* element_from_hash_batch on G1 and G2 against element_from_hash of the CPU pairing */
+    enum { H = 9, HL = 37 };
+    unsigned char msg[H * HL];
+    element_t G[H], ref1, ref2;
+    for (i = 0; i < H * HL; i++) msg[i] = (unsigned char)(i * 131 + 7);
+    element_init_G1(ref1, cpu); element_init_G2(ref2, cpu);
+    for (i = 0; i < H; i++) element_init_G1(G[i], gpu);
+    element_from_hash_batch(G, msg, HL, H);
+    for (i = 0; i < H; i++) {
+      element_from_hash(ref1, msg + i * HL, HL);
+      if (!same(G[i], ref1) && !(element_is0(ref1) && element_is0(G[i]))) { printf("G1 from_hash batch mismatch at %d\n", i); bad++; }
+      element_clear(G[i]);
+      element_init_G2(G[i], gpu);
+    }
+    element_from_hash_batch(G, msg, HL, H);
+    for (i = 0; i < H; i++) {
+      element_from_hash(ref2, msg + i * HL, HL);
+      if (!same(G[i], ref2)) { printf("G2 from_hash batch mismatch at %d\n", i); bad++; }
+      element_clear(G[i]);
+    }
+    element_clear(ref1); element_clear(ref2);
+  }
+  printf("shim_test: %s (%d batch pairings, prod, ragged prod 1+2+5, pp, identity, pow_zn, from_hash G1 / G2; G1 %d B, G2 %d B, GT %d B)\n",
          bad ? "FAILED" : "OK", n, pairing_length_in_bytes_G1(gpu), pairing_length_in_bytes_G2(gpu),
          pairing_length_in_bytes_GT(gpu));
   for (i = 0; i < n; i++) { element_clear(P[i]); element_clear(Q[i]); element_clear(E[i]); }

@@ -1,5 +1,5 @@
-"""Throughput of the batched group operations (element_pow_zn on G1 and GT) next to the compiled
-reference on the host cores.  One JSON line per (type, operation)."""
+"""Throughput of the batched group operations (element_pow_zn on G1 and GT, element_from_hash on G1 and G2,
+decompression on G2) next to the compiled reference on the host cores.  One JSON line per (type, operation)."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import multiprocessing as mp
@@ -84,6 +84,90 @@ def main():
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 3
         print(json.dumps({"type": wn, "op": "element_from_hash G1 (32-byte inputs)", "n": n, "ms": ms, "per_s": n / ms * 1e3}))
+
+    g2_lines(n, cores)
+
+
+def _cpu_g2(args):
+    """one worker's share of a G2 leg on the reference: (outputs, seconds of the reference work alone --
+    after the imports, the pairing init and one warm-up item)"""
+    name, op, data, n = args
+    from oracle import ref as R
+    from pbc_b200.params import PARAMS
+    rp = R.RefPairing(PARAMS[name])
+    run = (lambda d, k: rp.from_hash(R.G2, d, 32, k)) if op == "hash" else (lambda d, k: rp.decompress(R.G2, d, k))
+    run(data[:len(data) // n], 1)
+    t0 = time.perf_counter()
+    out = run(data, n)
+    return out, time.perf_counter() - t0
+
+
+# reference items per host core in the G2 legs: about a second of work each (one core does roughly 40 000
+# type f, 90 d159 and 15 g149 hashes per second)
+G2_CPU_PER_CORE = {"f": 8192, "d159": 96, "g149": 24}
+
+
+def _cpu_leg(pool, name, op, data, item, cores):
+    """run cores x G2_CPU_PER_CORE[name] items of `data` (item bytes each) on the reference, one share per
+    worker; returns (outputs, items/s over the cores = items / the slowest worker's work time, items/s of
+    one core = items / the summed work times)"""
+    per = G2_CPU_PER_CORE[name]
+    res = pool.map(_cpu_g2, [(name, op, data[c * per * item:(c + 1) * per * item], per) for c in range(cores)])
+    m = per * cores
+    return b"".join(r[0] for r in res), m / max(r[1] for r in res), m / sum(r[1] for r in res)
+
+
+def _time(fn, st):
+    import torch
+    for _ in range(2):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(st)
+    for _ in range(3):
+        fn()
+    e1.record(st)
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / 3
+
+
+def g2_lines(n, cores):
+    """element_from_hash on G2 (32-byte inputs) and G2 decompression (of those hashes, compressed on the
+    host) for f, d159 and g149; the reference runs a sample of G2_CPU_PER_CORE items per host core (worker
+    processes spawned fresh: this process has a CUDA context by now), timed on its work alone, and the
+    GPU's bytes for the same items are compared with its output"""
+    import numpy as np
+    import torch
+    from pbc_b200.pairing import Pairing
+    from pbc_b200.params import PARAMS
+    st = torch.cuda.current_stream()
+    pool = mp.get_context("spawn").Pool(cores)
+    for name in ("f", "d159", "g149"):
+        pr = Pairing(PARAMS[name])
+        H = np.random.default_rng(11).integers(0, 256, n * 32, dtype=np.uint8)
+        dH = torch.from_numpy(H).cuda()
+        dO = torch.empty(n * pr.g2_len, dtype=torch.uint8, device="cuda")
+        ms = _time(lambda: pr.g2_from_hash_device(dO.data_ptr(), dH.data_ptr(), 32, n, st.cuda_stream), st)
+        pts = bytes(dO.cpu().numpy().tobytes())
+        m = G2_CPU_PER_CORE[name] * cores
+        ref_out, rate, rate1 = _cpu_leg(pool, name, "hash", H.tobytes(), 32, cores)
+        print(json.dumps({"type": name, "op": "element_from_hash G2 (32-byte inputs)", "n": n, "ms": ms,
+                          "per_s": n / ms * 1e3, "cpu_reference_per_s": rate, "cpu_reference_per_core_per_s": rate1,
+                          "cpu_cores": cores, "cpu_sample": m, "parity_vs_reference": ref_out == pts[:m * pr.g2_len]}))
+        comp = pr.g2_compress(pts, n)
+        clen = len(comp) // n
+        # host buffers: the compressed items are clen (odd) bytes apart
+        pr.g2_decompress(comp[:clen * 1024], 1024)
+        t0 = time.perf_counter()
+        back = pr.g2_decompress(comp, n)
+        ms = (time.perf_counter() - t0) * 1e3
+        ref_out, rate, rate1 = _cpu_leg(pool, name, "dec", comp, clen, cores)
+        print(json.dumps({"type": name, "op": "element_from_bytes_compressed G2 (host buffers, copies included)",
+                          "n": n, "ms": ms, "per_s": n / ms * 1e3, "cpu_reference_per_s": rate,
+                          "cpu_reference_per_core_per_s": rate1, "cpu_cores": cores, "cpu_sample": m,
+                          "roundtrip": back == pts, "parity_vs_reference": ref_out == back[:m * pr.g2_len]}))
+    pool.close()
+    pool.join()
 
 
 if __name__ == "__main__":
